@@ -100,6 +100,20 @@ def cpu_baselines(rows: int) -> dict:
     out["scan"] = {"value": rows / t, "unit": "rows/s", "cores": 1, "kind": "port", "ms": t * 1e3, "sample": f"numpy cumsum of {rows} int64, best of 3"}
     t = _best(lambda: np.sum(x))
     out["reduce"] = {"value": rows / t, "unit": "rows/s", "cores": 1, "kind": "port", "ms": t * 1e3, "sample": f"numpy sum of {rows} int64, best of 3"}
+    # stream compaction: {int64, float64 with 50 % NaN} frame, 50 % boolean mask; drop_duplicates of the groupby key
+    u = datagen.fill(rows, SEED, 8 << 40, 1)
+    df = pd.DataFrame({"x": x, "p": np.where(datagen.fill(rows, SEED, 3 << 40, 4), u, np.nan)})
+    keep = u < 0.5
+    t = _best(lambda: df[keep])
+    out["apply_boolean_mask"] = {"value": rows / t, "unit": "rows/s", "cores": 1, "kind": "port", "ms": t * 1e3,
+                                 "sample": f"pandas boolean indexing of {rows} rows (int64 + float64 with 50 % NaN), 50 % mask, best of 3"}
+    t = _best(lambda: df.dropna(subset=["p"]))
+    out["drop_nulls"] = {"value": rows / t, "unit": "rows/s", "cores": 1, "kind": "port", "ms": t * 1e3,
+                         "sample": f"pandas dropna(subset=['p']) of {rows} rows, 50 % NaN, best of 3"}
+    ks = pd.Series(gk)
+    t = _best(lambda: ks.drop_duplicates())
+    out["distinct"] = {"value": rows / t, "unit": "rows/s", "cores": 1, "kind": "port", "ms": t * 1e3,
+                       "sample": f"pandas Series.drop_duplicates of {rows} int64 keys with {G} values, best of 3"}
     return out
 
 
@@ -179,6 +193,38 @@ def run(plc, _lib, n, peak_gbs, cpu_rows=10_000_000, with_cpu=True):
                                                 phases_ms=phases("groupby_partition", "groupby_aggregate"),
                                                 note="partition pass (one-sweep, mix64 top byte, value carried) + shared-memory aggregation per partition chunk")
     del k, v2, gb, reqs, keys_out
+    release()
+
+    # ---- stream compaction: {int64, float64 with 50 % nulls} table filtered by a 50 % BOOL8 mask / by its nulls; distinct on the
+    # groupby workload's key column (1e6 values) ----
+    x = _fill(_lib, torch.empty(n, dtype=torch.int64, device=dev), n, 7)
+    vmask = _fill(_lib, torch.empty((n + 31) // 32, dtype=torch.int32, device=dev), n, 3, kind=4)
+    pcol = plc.Column.from_torch(f, mask=vmask)
+    tbl = plc.Table([plc.Column.from_torch(x), pcol])
+    bm = f < 0.5
+    mcol = plc.Column.from_torch(bm)
+    sc = plc.stream_compaction
+    sw = 16  # bytes per row of the two columns
+    ms = profiled(lambda: sc.apply_boolean_mask(tbl, mcol))
+    s_ = sc.apply_boolean_mask(tbl, mcol).num_rows()
+    res["apply_boolean_mask_50pct"] = entry(ms, n, n * (1 + sw) + s_ * sw + n // 8 + s_ // 8, "apply_boolean_mask", kept=s_,
+                                            phases_ms=phases("compact", "gather"),
+                                            note="int64 + float64 (50 % nulls) table, 50 % BOOL8 mask; contract bytes: n(1 + 16) + 16s + validity in and out")
+    ms = profiled(lambda: sc.drop_nulls(tbl, [1]))
+    s_ = sc.drop_nulls(tbl, [1]).num_rows()
+    res["drop_nulls_50pct"] = entry(ms, n, n // 8 + n * sw + s_ * sw + s_ // 8, kept=s_, cpu_key="drop_nulls", phases_ms=phases("compact", "gather"),
+                                    note="same table, key = the float64 column; contract bytes: validity n/8 + 16n + 16s + s/8")
+    del tbl, pcol, mcol, bm, vmask, x
+    release()
+    k = _fill(_lib, torch.empty(n, dtype=torch.int64, device=dev), n, 9, kind=2, modulus=G)
+    kt = plc.Table([plc.Column.from_torch(k)])
+    args = (sc.DuplicateKeepOption.KEEP_ANY, plc.NullEquality.EQUAL, plc.NanEquality.ALL_EQUAL)
+    ms = profiled(lambda: sc.distinct(kt, [0], *args))
+    d = sc.distinct(kt, [0], *args).num_rows()
+    res["distinct_1e6_keys"] = entry(ms, n, 8 * n + 2 * n + 4 * d + 8 * d, "distinct", distinct_rows=d,
+                                     phases_ms=phases("distinct_insert", "distinct_mark", "compact", "gather"),
+                                     note="KEEP_ANY on the groupby key column; contract bytes: keys 8n + flags 2n + map 4d + keys out 8d")
+    del k, kt
     release()
 
     # ---- inner join (BASELINE configs[2]): |R| = |L| = n, 10 % of probe rows match exactly once; payload gather with 50 % nulls ----

@@ -161,6 +161,12 @@ _sig("b2_packed_size", [P(TableView), P(C.c_size_t)])
 _sig("b2_pack", [P(TableView), b2_stream, u8p, C.c_size_t, P(C.c_size_t), P(vp)])
 _sig("b2_pack_metadata", [P(TableView), vp, C.c_size_t, u8p, C.c_size_t, P(C.c_size_t)])
 _sig("b2_unpack", [u8p, C.c_size_t, vp, P(ColumnView), i32, P(i32), P(i32)])
+_sig("b2_apply_boolean_mask", [P(TableView), P(ColumnView), i32, b2_stream, P(vp)])
+_sig("b2_drop_nulls", [P(TableView), P(i32), i32, i32, b2_stream, P(vp)])
+_sig("b2_drop_nans", [P(TableView), P(i32), i32, i32, b2_stream, P(vp)])
+_sig("b2_unique", [P(TableView), P(i32), i32, i32, i32, b2_stream, P(vp)])
+_sig("b2_distinct", [P(TableView), P(i32), i32, i32, i32, i32, i32, b2_stream, P(vp)])
+_sig("b2_distinct_indices", [P(TableView), i32, i32, i32, b2_stream, P(vp)])
 _sig("b2_fill_splitmix64", [vp, C.c_int64, C.c_uint64, C.c_int64, i32, C.c_uint64, b2_stream])
 
 # every symbol the header declares, for the loader test
@@ -181,7 +187,8 @@ DECLARED_SYMBOLS = [
     "b2_partition_plan_create", "b2_partition_scatter", "b2_partition_scatter_staged", "b2_partition_plan_free", "b2_ipc_alloc", "b2_ipc_open", "b2_ipc_close",
     "b2_ipc_free", "b2_peer_copy", "b2_profile_get_over", "b2_hash_partition", "b2_partition_by_map", "b2_range_partition_counts", "b2_range_partition_scatter", "b2_packed_size", "b2_pack", "b2_pack_metadata", "b2_unpack", "b2_to_arrow_schema", "b2_to_arrow_device", "b2_to_arrow_host", "b2_from_arrow_device",
     "b2_from_arrow_host", "b2_arrow_schema_release", "b2_arrow_array_release",
-    "b2_fill_splitmix64",
+    "b2_fill_splitmix64", "b2_apply_boolean_mask", "b2_drop_nulls", "b2_drop_nans", "b2_unique", "b2_distinct",
+    "b2_distinct_indices",
 ]
 
 

@@ -3,6 +3,7 @@
 #pragma once
 #include <atomic>
 #include <cstdint>
+#include <cstring>
 #include <cuda_runtime.h>
 
 namespace b2 {
@@ -101,6 +102,40 @@ __device__ __forceinline__ T warp_sum(T v)
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// ---- decoupled look-back records (scan_kernel, compact_kernel) ------------------------------------
+// One 16-byte record per tile: {flag (0 nothing, 1 aggregate, 2 inclusive), pad, 8-byte value}. A 16-byte
+// aligned store is observed all-or-nothing by a 16-byte load, so the look-back needs no fences.
+struct scan_state {
+  uint4* rec;
+  uint32_t* ticket;
+};
+template <typename T>
+__device__ __forceinline__ void publish_rec(uint4* p, uint32_t flag, T v)
+{
+  unsigned long long bits = 0;
+  memcpy(&bits, &v, sizeof(T));
+#ifdef B2_EMU
+  *p = make_uint4(flag, 0u, (uint32_t)bits, (uint32_t)(bits >> 32));
+#else
+  asm volatile("st.volatile.global.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(flag), "r"(0u), "r"((uint32_t)bits),
+               "r"((uint32_t)(bits >> 32))
+               : "memory");
+#endif
+}
+template <typename T>
+__device__ __forceinline__ uint32_t read_rec(const uint4* p, T& v)
+{
+#ifdef B2_EMU
+  const uint4 r = *p;
+#else
+  uint4 r;
+  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "l"(p) : "memory");
+#endif
+  unsigned long long bits = (unsigned long long)r.z | ((unsigned long long)r.w << 32);
+  memcpy(&v, &bits, sizeof(T));
+  return r.x;
 }
 
 // ---- splitmix64 (SURVEY §8d generator) --------------------------------------------------------------

@@ -136,6 +136,47 @@ __device__ __forceinline__ slot_t load_slot(const slot_t* p)
   return s;
 }
 
+__device__ __forceinline__ slot_t cas128(slot_t* addr, const slot_t& expected, const slot_t& desired)
+{
+  uint64_t e0, e1, d0, d1, r0, r1;
+  memcpy(&e0, &expected, 8);
+  memcpy(&e1, reinterpret_cast<const char*>(&expected) + 8, 8);
+  memcpy(&d0, &desired, 8);
+  memcpy(&d1, reinterpret_cast<const char*>(&desired) + 8, 8);
+#ifdef B2_EMU
+  memcpy(&r0, addr, 8);
+  memcpy(&r1, reinterpret_cast<const char*>(addr) + 8, 8);
+  if (r0 == e0 && r1 == e1) {
+    memcpy(addr, &d0, 8);
+    memcpy(reinterpret_cast<char*>(addr) + 8, &d1, 8);
+  }
+#else
+  asm volatile(
+    "{\n .reg .b128 e, d, r;\n mov.b128 e, {%2, %3};\n mov.b128 d, {%4, %5};\n"
+    " atom.global.cas.b128 r, [%6], e, d;\n mov.b128 {%0, %1}, r;\n}"
+    : "=l"(r0), "=l"(r1)
+    : "l"(e0), "l"(e1), "l"(d0), "l"(d1), "l"(addr)
+    : "memory");
+#endif
+  slot_t out;
+  memcpy(&out, &r0, 8);
+  memcpy(reinterpret_cast<char*>(&out) + 8, &r1, 8);
+  return out;
+}
+
+__device__ __forceinline__ slot_t load_slot_volatile(const slot_t* p)
+{
+#ifdef B2_EMU
+  const uint4 v = *reinterpret_cast<const uint4*>(p);
+#else
+  uint4 v;
+  asm volatile("ld.volatile.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p) : "memory");
+#endif
+  slot_t s;
+  memcpy(&s, &v, 16);
+  return s;
+}
+
 inline int key_bytes(const std::vector<b2_column_view>& cols)
 {
   int total = 0;

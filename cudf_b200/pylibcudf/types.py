@@ -62,6 +62,11 @@ class NullEquality(enum.IntEnum):
     UNEQUAL = 1
 
 
+class NanEquality(enum.IntEnum):  # cudf::nan_equality (types.hpp)
+    ALL_EQUAL = 0
+    UNEQUAL = 1
+
+
 class Sorted(enum.IntEnum):
     NO = 0
     YES = 1

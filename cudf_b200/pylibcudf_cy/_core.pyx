@@ -369,6 +369,124 @@ def gather(Table source_table, Column gather_map, bounds_policy, stream=None, mr
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# stream compaction (python/pylibcudf/pylibcudf/stream_compaction.pyx; cpp/include/cudf/stream_compaction.hpp)
+# ---------------------------------------------------------------------------------------------------------------------
+cdef class _KeyIndices:
+    """A C array of int32 key column indices (valid while the object lives)."""
+    cdef int32_t* p
+    cdef int32_t n
+
+    def __cinit__(self, keys):
+        keys = [int(k) for k in keys]
+        self.n = len(keys)
+        self.p = <int32_t*>calloc(max(self.n, 1), sizeof(int32_t))
+        if self.p == NULL:
+            raise MemoryError()
+        for j in range(self.n):
+            self.p[j] = keys[j]
+
+    def __dealloc__(self):
+        free(self.p)
+
+
+cdef Table _mask_call(Table input, Column mask, int32_t deletion, stream):
+    cdef _TableView tv = _TableView.of(input)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_table* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_apply_boolean_mask(&tv.tv, &mask.v, deletion, s, &out)
+    check(st)
+    return Table.from_handle(out)
+
+
+def apply_boolean_mask(Table source_table, Column boolean_mask, stream=None, mr=None):
+    """Rows where `boolean_mask` (BOOL8) is valid and true, in input order."""
+    return _mask_call(source_table, boolean_mask, 0, stream)
+
+
+def apply_deletion_mask(Table input, Column deletion_mask, stream=None, mr=None):  # noqa: A002
+    """Rows where `deletion_mask` (BOOL8) is valid and false, in input order."""
+    return _mask_call(input, deletion_mask, 1, stream)
+
+
+cdef Table _threshold_call(Table input, keys, keep_threshold, bint nans, stream):
+    cdef _TableView tv = _TableView.of(input)
+    cdef _KeyIndices k = _KeyIndices(keys)
+    cdef int32_t thr = k.n if keep_threshold is None else int(keep_threshold)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_table* out = NULL
+    cdef b2_status st
+    with nogil:
+        if nans:
+            st = b2_drop_nans(&tv.tv, k.p, k.n, thr, s, &out)
+        else:
+            st = b2_drop_nulls(&tv.tv, k.p, k.n, thr, s, &out)
+    check(st)
+    return Table.from_handle(out)
+
+
+def drop_nulls(Table source_table, keys, keep_threshold=None, stream=None, mr=None):
+    """Rows with at least `keep_threshold` (default: all) valid columns among `keys`."""
+    return _threshold_call(source_table, keys, keep_threshold, False, stream)
+
+
+def drop_nans(Table source_table, keys, keep_threshold=None, stream=None, mr=None):
+    """Rows with at least `keep_threshold` (default: all) non-NaN columns among the float `keys`; a null is not NaN."""
+    return _threshold_call(source_table, keys, keep_threshold, True, stream)
+
+
+def unique(Table input, keys, keep, nulls_equal, stream=None, mr=None):  # noqa: A002
+    """Drops consecutive duplicate rows of the `keys` columns."""
+    cdef _TableView tv = _TableView.of(input)
+    cdef _KeyIndices k = _KeyIndices(keys)
+    cdef int32_t kp = int(keep), ne = int(nulls_equal)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_table* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_unique(&tv.tv, k.p, k.n, kp, ne, s, &out)
+    check(st)
+    return Table.from_handle(out)
+
+
+cdef Table _distinct_call(Table input, keys, keep, nulls_equal, nans_equal, int32_t stable, stream):
+    cdef _TableView tv = _TableView.of(input)
+    cdef _KeyIndices k = _KeyIndices(keys)
+    cdef int32_t kp = int(keep), ne = int(nulls_equal), nn = int(nans_equal)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_table* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_distinct(&tv.tv, k.p, k.n, kp, ne, nn, stable, s, &out)
+    check(st)
+    return Table.from_handle(out)
+
+
+def distinct(Table input, keys, keep, nulls_equal, nans_equal, stream=None, mr=None):  # noqa: A002
+    """One row per set of equal `keys` rows; the order is unspecified (here: input order)."""
+    return _distinct_call(input, keys, keep, nulls_equal, nans_equal, 0, stream)
+
+
+def stable_distinct(Table input, keys, keep, nulls_equal, nans_equal, stream=None, mr=None):  # noqa: A002
+    """The rows of `distinct`, in input order."""
+    return _distinct_call(input, keys, keep, nulls_equal, nans_equal, 1, stream)
+
+
+def distinct_indices(Table input, keep, nulls_equal, nans_equal, stream=None, mr=None):  # noqa: A002
+    """INT32 indices of the rows `distinct` keeps over all columns of `input`, ascending."""
+    cdef _TableView tv = _TableView.of(input)
+    cdef int32_t kp = int(keep), ne = int(nulls_equal), nn = int(nans_equal)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_distinct_indices(&tv.tv, kp, ne, nn, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # joins (python/pylibcudf/pylibcudf/join.pyx:63-205; cudf::hash_join)
 # ---------------------------------------------------------------------------------------------------------------------
 ctypedef b2_status (*free_join_fn)(const b2_table_view*, const b2_table_view*, int32_t, b2_stream, b2_column**, b2_column**) noexcept nogil

@@ -134,6 +134,20 @@ cdef extern from "cudf_b200.h" nogil:
     b2_status b2_partition_by_map(const b2_table_view* input, const b2_column_view* partition_map, int32_t num_partitions,
                                   b2_stream stream, b2_table** out, int32_t* out_offsets)
 
+    # stream compaction (cpp/include/cudf/stream_compaction.hpp)
+    b2_status b2_apply_boolean_mask(const b2_table_view* input, const b2_column_view* mask, int32_t deletion, b2_stream stream,
+                                    b2_table** out)
+    b2_status b2_drop_nulls(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep_threshold,
+                            b2_stream stream, b2_table** out)
+    b2_status b2_drop_nans(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep_threshold,
+                           b2_stream stream, b2_table** out)
+    b2_status b2_unique(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep, int32_t nulls_equal,
+                        b2_stream stream, b2_table** out)
+    b2_status b2_distinct(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep, int32_t nulls_equal,
+                          int32_t nans_equal, int32_t stable, b2_stream stream, b2_table** out)
+    b2_status b2_distinct_indices(const b2_table_view* input, int32_t keep, int32_t nulls_equal, int32_t nans_equal,
+                                  b2_stream stream, b2_column** out)
+
     # cudf::pack / unpack (cpp/include/cudf/contiguous_split.hpp:233-317)
     void* b2_buffer_data(const b2_buffer* buf)
     size_t b2_buffer_size(const b2_buffer* buf)

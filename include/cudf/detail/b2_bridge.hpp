@@ -101,6 +101,7 @@ using bitmask_type = uint32_t;
 enum class order : bool { ASCENDING, DESCENDING };
 enum class null_policy : bool { EXCLUDE, INCLUDE };
 enum class null_equality : bool { EQUAL, UNEQUAL };
+enum class nan_equality : int32_t { ALL_EQUAL, UNEQUAL };  // types.hpp: NaN == NaN, or every NaN distinct
 enum class null_order : bool { AFTER, BEFORE };
 enum class sorted : bool { NO, YES };
 enum class mask_state : int32_t { UNALLOCATED, UNINITIALIZED, ALL_VALID, ALL_NULL };
@@ -836,6 +837,103 @@ inline table_view unpack(uint8_t const* metadata, size_t metadata_size, uint8_t 
 inline table_view unpack(packed_columns const& input)
 {
   return unpack(input.metadata->data(), input.metadata->size(), static_cast<uint8_t const*>(input.gpu_data->data()));
+}
+
+// ------------------------------------------------------------------------------------------------
+// stream_compaction.hpp (cpp/include/cudf/stream_compaction.hpp:73-390): fixed-width columns, at most 8 key columns
+// ------------------------------------------------------------------------------------------------
+enum class duplicate_keep_option : int32_t { KEEP_ANY = 0, KEEP_FIRST, KEEP_LAST, KEEP_NONE };
+namespace detail {
+template <typename F>
+inline std::unique_ptr<table> table_call(F&& f)
+{
+  b2_table* out = nullptr;
+  check(f(&out));
+  return table::from_handle(out);
+}
+}  // namespace detail
+inline std::unique_ptr<table> drop_nulls(table_view const& input, std::vector<size_type> const& keys, size_type keep_threshold,
+                                         rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                         rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  return detail::table_call([&](b2_table** o) {
+    return b2_drop_nulls(&tv, keys.data(), static_cast<int32_t>(keys.size()), keep_threshold, stream.value(), o);
+  });
+}
+inline std::unique_ptr<table> drop_nulls(table_view const& input, std::vector<size_type> const& keys,
+                                         rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                         rmm::device_async_resource_ref mr = cudf::get_current_device_resource_ref())
+{
+  return drop_nulls(input, keys, static_cast<size_type>(keys.size()), stream, mr);
+}
+inline std::unique_ptr<table> drop_nans(table_view const& input, std::vector<size_type> const& keys, size_type keep_threshold,
+                                        rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                        rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  return detail::table_call([&](b2_table** o) {
+    return b2_drop_nans(&tv, keys.data(), static_cast<int32_t>(keys.size()), keep_threshold, stream.value(), o);
+  });
+}
+inline std::unique_ptr<table> drop_nans(table_view const& input, std::vector<size_type> const& keys,
+                                        rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                        rmm::device_async_resource_ref mr = cudf::get_current_device_resource_ref())
+{
+  return drop_nans(input, keys, static_cast<size_type>(keys.size()), stream, mr);
+}
+inline std::unique_ptr<table> apply_boolean_mask(table_view const& input, column_view const& boolean_mask,
+                                                 rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                 rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  return detail::table_call([&](b2_table** o) { return b2_apply_boolean_mask(&tv, &boolean_mask.native(), 0, stream.value(), o); });
+}
+inline std::unique_ptr<table> apply_deletion_mask(table_view const& input, column_view const& deletion_mask,
+                                                  rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                  rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  return detail::table_call([&](b2_table** o) { return b2_apply_boolean_mask(&tv, &deletion_mask.native(), 1, stream.value(), o); });
+}
+inline std::unique_ptr<table> unique(table_view const& input, std::vector<size_type> const& keys, duplicate_keep_option keep,
+                                     null_equality nulls_equal = null_equality::EQUAL,
+                                     rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                     rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  return detail::table_call([&](b2_table** o) {
+    return b2_unique(&tv, keys.data(), static_cast<int32_t>(keys.size()), static_cast<int32_t>(keep), static_cast<int32_t>(nulls_equal),
+                     stream.value(), o);
+  });
+}
+#define CUDF_B2_DISTINCT(NAME, STABLE)                                                                                              \
+  inline std::unique_ptr<table> NAME(table_view const& input, std::vector<size_type> const& keys,                                   \
+                                     duplicate_keep_option keep = duplicate_keep_option::KEEP_ANY,                                  \
+                                     null_equality nulls_equal = null_equality::EQUAL, nan_equality nans_equal = nan_equality::ALL_EQUAL, \
+                                     rmm::cuda_stream_view stream = cudf::get_default_stream(),                                     \
+                                     rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())                      \
+  {                                                                                                                                 \
+    auto tv = input.native();                                                                                                       \
+    return detail::table_call([&](b2_table** o) {                                                                                   \
+      return b2_distinct(&tv, keys.data(), static_cast<int32_t>(keys.size()), static_cast<int32_t>(keep),                           \
+                         static_cast<int32_t>(nulls_equal), static_cast<int32_t>(nans_equal), STABLE, stream.value(), o);           \
+    });                                                                                                                             \
+  }
+CUDF_B2_DISTINCT(distinct, 0)
+CUDF_B2_DISTINCT(stable_distinct, 1)
+#undef CUDF_B2_DISTINCT
+inline std::unique_ptr<column> distinct_indices(table_view const& input, duplicate_keep_option keep = duplicate_keep_option::KEEP_ANY,
+                                                null_equality nulls_equal = null_equality::EQUAL,
+                                                nan_equality nans_equal = nan_equality::ALL_EQUAL,
+                                                rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  auto tv = input.native();
+  b2_column* out = nullptr;
+  detail::check(b2_distinct_indices(&tv, static_cast<int32_t>(keep), static_cast<int32_t>(nulls_equal), static_cast<int32_t>(nans_equal),
+                                    stream.value(), &out));
+  return std::make_unique<column>(out);
 }
 
 }  // namespace cudf

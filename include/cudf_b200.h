@@ -306,6 +306,37 @@ B2_API b2_status b2_hash_partition(const b2_table_view* input, const b2_table_vi
 B2_API b2_status b2_partition_by_map(const b2_table_view* input, const b2_column_view* partition_map, int32_t num_partitions,
                                      b2_stream stream, b2_table** out, int32_t* out_offsets);
 
+/* ---- stream compaction: cpp/include/cudf/stream_compaction.hpp, cpp/src/stream_compaction/*.  Fixed-width keys, at most
+ *      8 key columns.  keep = cudf::duplicate_keep_option (0 ANY, 1 FIRST, 2 LAST, 3 NONE); nulls_equal = null_equality
+ *      (0 EQUAL, 1 UNEQUAL); nans_equal = cudf::nan_equality (0 ALL_EQUAL, 1 UNEQUAL).  A key index outside the table is
+ *      OUT_OF_RANGE (table_view::select). -------------------------------------------------------------------------------- */
+enum { B2_KEEP_ANY = 0, B2_KEEP_FIRST = 1, B2_KEEP_LAST = 2, B2_KEEP_NONE = 3 };
+enum { B2_NANS_ALL_EQUAL = 0, B2_NANS_UNEQUAL = 1 };
+/* cudf::apply_boolean_mask (deletion = 0; apply_boolean_mask.cu:22-117) / cudf::apply_deletion_mask (deletion = 1): keeps
+ * row i when mask[i] is valid and true (false), in input order.  The mask must be BOOL8 (LOGIC) and, when the table has
+ * rows, have as many rows (LOGIC); an empty mask gives an empty table of the input's types. */
+B2_API b2_status b2_apply_boolean_mask(const b2_table_view* input, const b2_column_view* mask, int32_t deletion, b2_stream stream,
+                                       b2_table** out);
+/* cudf::drop_nulls (drop_nulls.cu:57-66): keeps the rows with at least keep_threshold valid key columns.  No keys, no rows
+ * or no nulls in the keys: a copy of the input. */
+B2_API b2_status b2_drop_nulls(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep_threshold,
+                               b2_stream stream, b2_table** out);
+/* cudf::drop_nans (drop_nans.cu:78-100): keeps the rows with at least keep_threshold non-NaN key columns (a null is not
+ * NaN).  A non-float key column is LOGIC. */
+B2_API b2_status b2_drop_nans(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep_threshold,
+                              b2_stream stream, b2_table** out);
+/* cudf::unique (unique.cu:42-121): drops consecutive duplicate key rows (ANY = FIRST; NONE drops every row with an equal
+ * neighbour); NaN == NaN, -0 == +0. */
+B2_API b2_status b2_unique(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep, int32_t nulls_equal,
+                           b2_stream stream, b2_table** out);
+/* cudf::distinct / cudf::stable_distinct (distinct.cu:76-200, stable_distinct.cu): one row per set of equal key rows (NONE:
+ * only the rows whose key occurs once).  Both return the rows in input order; `stable` is accepted for symmetry. */
+B2_API b2_status b2_distinct(const b2_table_view* input, const int32_t* keys, int32_t num_keys, int32_t keep, int32_t nulls_equal,
+                             int32_t nans_equal, int32_t stable, b2_stream stream, b2_table** out);
+/* cudf::distinct_indices (distinct.cu:76-200, 185-200): INT32 indices of the kept rows over all columns, ascending. */
+B2_API b2_status b2_distinct_indices(const b2_table_view* input, int32_t keep, int32_t nulls_equal, int32_t nans_equal,
+                                     b2_stream stream, b2_column** out);
+
 /* Two-phase form of b2_partition for the fused partition + exchange: the plan holds the bucket id and the
  * stable in-bucket rank of every row; out_counts[b] = rows of bucket b.  b2_partition_scatter then writes one
  * fixed-width column straight to P destination base addresses — local buffers or PEER device memory mapped with

@@ -56,9 +56,11 @@ struct gb_ctl {
   unsigned int overflow;
 };
 
-// order-preserving double <-> int64 (for MIN/MAX of floats with integer atomics)
+// order-preserving double <-> int64 (for MIN/MAX of floats with integer atomics). Every NaN maps to the positive quiet NaN,
+// which orders above +inf: MIN / MAX rank NaN above +inf whatever its sign, as scan_reduce.cu's binop does.
 __device__ __forceinline__ long long f64_to_ordered(double v)
 {
+  if (v != v) return 0x7ff8000000000000ll;
   long long b = __double_as_longlong(v);
   return b >= 0 ? b : (b ^ 0x7fffffffffffffffll);
 }
@@ -168,7 +170,12 @@ __global__ void __launch_bounds__(256) groupby_kernel(key_cols kc, int64_t n, bo
               unsigned long long hu = 0;
               double hf = 0;
               load_value(op, held + op.offset, hi_, hu, hf);
-              if (op.acc == ACC_F64) better = (want_max ? fv > hf : fv < hf) || (fv == hf && r < held);
+              if (op.acc == ACC_F64) {
+                // the order of MIN / MAX: NaN ranks above +inf, and NaNs tie
+                const bool fn = fv != fv, hn = hf != hf;
+                const bool beats = want_max ? (!hn && (fn || fv > hf)) : (!fn && (hn || fv < hf));
+                better = beats || ((fn ? hn : fv == hf) && r < held);
+              }
               else if (op.acc == ACC_I64) better = (want_max ? iv > hi_ : iv < hi_) || (iv == hi_ && r < held);
               else better = (want_max ? uv > hu : uv < hu) || (uv == hu && r < held);
             }
@@ -972,12 +979,13 @@ __global__ void group_heads_kernel(key_cols kc, const int32_t* __restrict__ orde
 // Element = (value as 8-byte accumulator, valid flag); op: SUM / MIN / MAX / COUNT.
 constexpr int SEG_TILE = 2048;
 
+// MIN / MAX rank NaN above +inf (scan_reduce.cu's binop), so NaN is MIN's identity for doubles
 template <typename A, int OPK>
 __device__ __forceinline__ A seg_apply(A a, A b)
 {
   if (OPK == OPK_SUM) return a + b;
-  if (OPK == OPK_MIN) return b < a ? b : a;
-  return a < b ? b : a;
+  if (OPK == OPK_MIN) return (b < a || a != a) ? b : a;  // a != a: a is NaN (false for integers)
+  return (a < b || b != b) ? b : a;
 }
 template <typename A, int OPK>
 __device__ __forceinline__ A seg_identity()
@@ -986,7 +994,7 @@ __device__ __forceinline__ A seg_identity()
   if (OPK == OPK_MIN) return sizeof(A) == 8 && ((A)-1 < A(0)) ? (A)INT64_MAX : (A)~0ull;
   return ((A)-1 < A(0)) ? (A)INT64_MIN : A(0);
 }
-template <> __device__ __forceinline__ double seg_identity<double, OPK_MIN>() { return __longlong_as_double(0x7ff0000000000000ll); }
+template <> __device__ __forceinline__ double seg_identity<double, OPK_MIN>() { return __longlong_as_double(0x7ff8000000000000ll); }
 template <> __device__ __forceinline__ double seg_identity<double, OPK_MAX>() { return __longlong_as_double(0xfff0000000000000ll); }
 
 template <typename A>

@@ -138,16 +138,17 @@ def aggregate(key_cols, requests, null_handling=EXCLUDE):
                 per.append((out, None if (kind == NUNIQUE or ok.all()) else ok))
                 continue
             if kind in (ARGMAX, ARGMIN):
-                # global_memory_aggregator.cuh:155-200 (strict > / < comparisons: a NaN never displaces a holder)
+                # global_memory_aggregator.cuh:155-200, in the order of MIN / MAX: NaN ranks above +inf and NaNs tie
                 out = np.full(ng, -1, np.int32)
                 xv, xg, xr = v[m], gid[m], rows[m]
+                rank = lambda x: (1, 0.0) if x != x else (0, x)
                 for val, g, r in zip(xv.tolist(), xg.tolist(), xr.tolist()):
                     h = out[g]
                     if h < 0:
                         out[g] = r
                         continue
-                    hv = vals[h].item()
-                    if (val > hv if kind == ARGMAX else val < hv) or (val == hv and r < h):
+                    a, b = rank(val), rank(vals[h].item())
+                    if (a > b if kind == ARGMAX else a < b) or (a == b and r < h):
                         out[g] = r
                 per.append((out, (vc > 0) if has_nulls else None))
                 continue
@@ -172,8 +173,9 @@ def aggregate(key_cols, requests, null_handling=EXCLUDE):
                     np.multiply.at(acc, xg, xv.astype(acc.dtype))
                     out = acc.astype(rdt)
                 elif kind == MIN:
-                    big = np.full(ng, np.inf if rdt.kind == "f" else (np.iinfo(rdt).max if rdt != np.bool_ else True), dtype=rdt)
-                    np.minimum.at(big, xg, xv)
+                    # NaN ranks above +inf (fmin drops it while a number is there); MAX's np.maximum propagates it
+                    big = np.full(ng, np.nan if rdt.kind == "f" else (np.iinfo(rdt).max if rdt != np.bool_ else True), dtype=rdt)
+                    np.fmin.at(big, xg, xv)
                     out = big
                 elif kind == MAX:
                     small = np.full(ng, -np.inf if rdt.kind == "f" else (np.iinfo(rdt).min if rdt != np.bool_ else False), dtype=rdt)

@@ -44,7 +44,8 @@ def _fold(kind, x, acc_dtype):
                 return np.bool_(x.all())
             return x.prod(dtype=acc_dtype) if len(x) else acc_dtype.type(1)
         if kind == MIN:
-            return x.min() if len(x) else _identity(MIN, acc_dtype)
+            # NaN ranks above +inf: fmin is NaN only when every value is NaN (maximum propagates NaN already)
+            return np.fmin.reduce(x) if len(x) else _identity(MIN, acc_dtype)
         if kind == MAX:
             return x.max() if len(x) else _identity(MAX, acc_dtype)
     raise ValueError(kind)
@@ -111,13 +112,16 @@ def scan(values, valid, kind, inclusive=True, null_handling=EXCLUDE):
         elif kind == PRODUCT:
             r = np.cumprod(x, dtype=dt) if dt != np.bool_ else np.logical_and.accumulate(x)
         elif kind == MIN:
-            r = np.minimum.accumulate(x)
+            # NaN ranks above +inf, so a prefix is NaN only while all its valid values are; nulls take NaN, the top
+            r = np.fmin.accumulate(np.where(v, values, np.nan).astype(dt) if dt.kind == "f" else x)
         elif kind == MAX:
             r = np.maximum.accumulate(x)
         else:
             raise RuntimeError("Unsupported aggregation operator for scan")
     if not inclusive:
         r = np.concatenate([np.array([ident], dtype=dt), r[:-1]]).astype(dt) if n else r
+        if kind == MIN and dt.kind == "f":
+            r[: (int(np.argmax(v)) if v.any() else n) + 1] = ident  # an empty prefix: +inf, as in the reference
     return r, out_valid
 
 

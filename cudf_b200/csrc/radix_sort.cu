@@ -1890,7 +1890,9 @@ column_ptr sort_by_key_carry(const b2_column_view& keys, const b2_column_view& v
     dbuf a(sizeof(UK) * n, stream), b(sizeof(UK) > 1 ? sizeof(UK) * n : 0, stream);
     if constexpr (sizeof(UK) == 8) {
       // B2_SORT_CFG on the payload-carrying kernel: 10 = round-1 ranking (no extra __syncwarp, offsets by LDS + STS), 11 = race-free
-      // ranking with LDS + STS offsets; the default is race-free + one ATOMS.ADD per digit run
+      // ranking with LDS + STS offsets, 13 = the 384 x 16 tile with two CTAs per SM and per-thread key loads (the default of 4-byte
+      // payloads); the default is race-free + one ATOMS.ADD per digit run. 8-byte payloads take 512 x 20 tiles, one CTA per SM,
+      // keys by one bulk async copy per tile: 13.2 instead of 16.0 ms per 1e9-row pass on the H100 (DESIGN.md §4.1)
       switch (sort_cfg_env()) {
         case 10:
           run_radix_cfg<UK, 384, 16, 2, VT, true, false, false, false>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(), b.as<UK>(),
@@ -1902,10 +1904,20 @@ column_ptr sort_by_key_carry(const b2_column_view& keys, const b2_column_view& v
                                                                       out->data.as<int32_t>(), vtmp.as<int32_t>(), nullptr, 0, n, kind,
                                                                       !ascending, true, stream, 0, 7, false, vin);
           break;
-        default:
+        case 13:
           run_radix_cfg<UK, 384, 16, 2, VT, true>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(), b.as<UK>(),
                                                   out->data.as<int32_t>(), vtmp.as<int32_t>(), nullptr, 0, n, kind, !ascending, true,
                                                   stream, 0, 7, false, vin);
+          break;
+        default:
+          if constexpr (sizeof(VT) == 8)
+            run_radix_cfg<UK, 512, 20, 1, VT, true, false, true, true, true>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(),
+                                                                             b.as<UK>(), out->data.as<int32_t>(), vtmp.as<int32_t>(), nullptr,
+                                                                             0, n, kind, !ascending, true, stream, 0, 7, false, vin);
+          else
+            run_radix_cfg<UK, 384, 16, 2, VT, true>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(), b.as<UK>(),
+                                                    out->data.as<int32_t>(), vtmp.as<int32_t>(), nullptr, 0, n, kind, !ascending, true,
+                                                    stream, 0, 7, false, vin);
       }
     } else
       run_radix_cfg<UK, 512, 16, 1, VT, true>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(), b.as<UK>(),

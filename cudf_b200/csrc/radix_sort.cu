@@ -64,6 +64,12 @@ struct sort_ctl {
   int32_t need_low;            // 1: phase 1 could not decide, the low digits' histograms are required
   int32_t fix_fast;            // hybrid plan: which segment_fix_kernel instantiation runs (0: plain walks, 1: branch-free first neighbours)
   unsigned long long vary;     // OR of (key ^ first key) over the input
+  // range tier of the hybrid plan (see range_sort_kernel): the executed passes sort only the range id = (key >> range_shift) &
+  // (2^range_bits - 1); each range is then sorted in shared memory by the digits in range_digits and the segment walk
+  int32_t range;
+  int32_t range_shift;
+  int32_t range_bits;
+  uint32_t range_digits;       // bit p: digit p is ranked inside the ranges
 };
 
 template <typename UK>
@@ -237,8 +243,12 @@ constexpr int HYB_MIN_SAVED_PASSES = 2;
 // known to be constant or not from ctl->vary; if the hybrid plan can stop within the top digits it is final, otherwise
 // ctl->need_low is raised, the gated second histogram counts digits 0..3 and phase 2 plans with everything (phase 2 returns
 // at once when phase 1 was final).
+// range_allowed (hybrid plan only): the caller can run range_sort_kernel. The plan then stops the passes at the top one or two
+// adjacent non-trivial digits once the expected range, n * prod coll, stays below RANGE_CAP by five standard deviations of a
+// uniform spread (1e9 uniform keys: 15 259 + 5 * 124 rows against 16 384), and at least one digit is left to rank in the ranges.
+constexpr int RANGE_CAP = 16384;  // rows of one range: range_sort_kernel holds its keys in 128 KB of shared memory
 __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint32_t n, int raw, int pre_idx_buf,
-                            sort_ctl* ctl, int first_pass, int last_pass, int hyb_allowed, int phase = 0)
+                            sort_ctl* ctl, int first_pass, int last_pass, int hyb_allowed, int phase = 0, int range_allowed = 0)
 {
   __shared__ uint32_t warp_tot[8];
   __shared__ int triv[8];
@@ -305,6 +315,34 @@ __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint3
       }
       ctl->need_low = 0;
     }
+    int range = 0, range_low = 0, range_bits = 0;
+    uint32_t range_digits = 0;
+    if (hybrid && range_allowed) {
+      double e = (double)n;
+      for (int p = npass - 1; p > low && range_bits < 16; --p) {
+        if (triv[p]) {
+          if (range_bits == 0) continue;
+          break;  // the range id is one run of adjacent digits
+        }
+        e *= coll[p];
+        range_bits += RADIX_BITS;
+        if (e + 5.0 * sqrt(e) <= (double)RANGE_CAP) {
+          for (int q = low; q < p; ++q) range_digits |= triv[q] ? 0u : 1u << q;
+          range = range_digits != 0;
+          range_low = p;
+          break;
+        }
+      }
+      if (range) {
+        for (int q = 0; q < range_low; ++q) triv[q] = 1;
+        nexec = 0;
+        for (int q = 0; q < npass; ++q) nexec += triv[q] ? 0 : 1;
+      }
+    }
+    ctl->range        = range;
+    ctl->range_shift  = range_low * RADIX_BITS;
+    ctl->range_bits   = range ? range_bits : 0;
+    ctl->range_digits = range_digits;
     ctl->hybrid    = hybrid;
     // expected rows per segment decides the fix-up flavour: mostly single-row segments (1e9 uniform keys: 0.23) take the
     // plain walks, ~2-row segments (a rank's shard of the sharded sort: 1.9) the branch-free form
@@ -451,8 +489,117 @@ constexpr bool EMU_BUILD = true;
 #else
 constexpr bool EMU_BUILD = false;
 #endif
-// RMW (default): the leader advances the warp's running digit offset with one ATOMS.ADD (returning the old value) instead of
+// Warp-private digit histogram of the first `nit` of a thread's IPT items (shared-memory atomics, no dependency chain);
+// returns the number of distinct digits among the warp's items, which picks the ranking flavour of warp_rank.
+template <int IPT, typename DigitAt>
+__device__ __forceinline__ int warp_digit_counts(const DigitAt& digit_at, int nit, int lane, uint32_t* my_hist)
+{
+#pragma unroll
+  for (int i = 0; i < IPT; ++i)
+    if (i < nit) atomicAdd(&my_hist[digit_at(i)], 1u);
+  __syncwarp();
+  int distinct = 0;
+#pragma unroll
+  for (int j = 0; j < RADIX / 32; ++j) distinct += my_hist[j * 32 + lane] != 0u;
+  return __reduce_add_sync(0xffffffffu, distinct);
+}
+
+// Stable rank of a thread's first `nit` items (item i of lane l comes after item i of lanes < l and after every item < i):
+// pos[i] = my_hist[digit] + rank among the warp's earlier items of that digit; my_hist[d] advances past the warp's digit-d items.
+// my_hist must hold the warp's starting offset of every digit, and my_bm must be zero (it is left zero).
+// Peer masks (lanes of the warp holding the same digit; scripts/ubench/rank_probe.cu compares the strategies):
+// MATCH.ANY is cheap only when the warp holds few distinct digits, the shared-memory atomicOr bitmap costs
+// about the same at any digit mix.  Hence: bitmap for the general case, MATCH.ANY when the warp holds only a handful of distinct digits.
+// All MATCH ops are issued first (independent, pipelined); only the counter chain is serial.
+// SAFE: a __syncwarp between the followers' read of the peer bitmap and the leader's clear — race-free under
+// independent thread scheduling (compute-sanitizer racecheck flags the form without it).
+// RMW: the leader advances the warp's running digit offset with one ATOMS.ADD (returning the old value) instead of
 // LDS + STS — one shared-memory operation less per key in a kernel bound by shared-memory wavefronts.
+template <int IPT, bool SAFE, bool RMW, typename DigitAt>
+__device__ __forceinline__ void warp_rank(const DigitAt& digit_at, int nit, int distinct, int lane, uint32_t* my_hist, uint32_t* my_bm,
+                                          uint32_t (&pos)[IPT])
+{
+  if (distinct > 4) {
+#pragma unroll
+    for (int i = 0; i < IPT; ++i) {
+      if (i >= nit) break;
+      const unsigned d = digit_at(i);
+      atomicOr(&my_bm[d], 1u << lane);
+      __syncwarp();
+      const unsigned peers = my_bm[d];
+      const unsigned lt = __popc(peers & lanemask_lt());
+      uint32_t prev = 0;
+      // The emulator (tests/emu) runs the lanes of a warp one after the other between rendezvous points, so the
+      // leader's clear below would be seen by the followers' read above. On the GPU the warp executes this
+      // straight-line stretch converged (validated on hardware); SAFE is the formally race-free variant.
+      if constexpr (SAFE || EMU_BUILD) __syncwarp();
+      if (lt == 0) {
+        if constexpr (RMW) {
+          prev = atomicAdd(&my_hist[d], (uint32_t)__popc(peers));
+        } else {
+          prev = my_hist[d];
+          my_hist[d] = prev + __popc(peers);
+        }
+        my_bm[d] = 0;
+      }
+      __syncwarp();
+      prev = __shfl_sync(0xffffffffu, prev, __ffs(peers) - 1);
+      pos[i] = prev + lt;
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < IPT; ++i) {
+      if (i >= nit) break;
+      const unsigned d = digit_at(i);
+      const unsigned peers = __match_any_sync(0xffffffffu, d);
+      const unsigned lt = __popc(peers & lanemask_lt());
+      uint32_t prev = 0;
+      if (lt == 0) {
+        prev = my_hist[d];
+        my_hist[d] = prev + __popc(peers);
+      }
+      __syncwarp();
+      prev = __shfl_sync(0xffffffffu, prev, __ffs(peers) - 1);
+      pos[i] = prev + lt;
+    }
+  }
+}
+
+// One bulk async copy (cp.async.bulk, the 1-D TMA path: UBLKCP in SASS) of `bytes` (a multiple of 16, both addresses 16-byte
+// aligned) into shared memory, completing on the mbarrier at shared address `mbar` (initialised with one arrival), and the
+// wait for it (phase 0). Not in the emulator build, which replays the data movement with ordinary loads.
+__device__ __forceinline__ void mbar_init_one(uint32_t mbar)
+{
+#ifndef B2_EMU
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar) : "memory");
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+#else
+  (void)mbar;
+#endif
+}
+__device__ __forceinline__ void bulk_copy_to_smem(void* sdst, const void* gsrc, uint32_t bytes, uint32_t mbar)
+{
+#ifndef B2_EMU
+  const uint32_t dst = (uint32_t)__cvta_generic_to_shared(sdst);
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(bytes) : "memory");
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(gsrc), "r"(bytes),
+               "r"(mbar)
+               : "memory");
+#else
+  (void)sdst; (void)gsrc; (void)bytes; (void)mbar;
+#endif
+}
+__device__ __forceinline__ void mbar_wait_phase0(uint32_t mbar)
+{
+#ifndef B2_EMU
+  asm volatile("{\n .reg .pred p;\n BULK_WAIT:\n mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n @p bra BULK_DONE;\n bra BULK_WAIT;\n BULK_DONE:\n}" ::"r"(mbar)
+               : "memory");
+#else
+  (void)mbar;
+#endif
+}
+
+// RMW (default): see warp_rank.
 // BULK: full, 16-byte aligned key tiles arrive in shared memory through ONE bulk async copy (cp.async.bulk, the 1-D TMA
 // path: UBLKCP in SASS) signalled by an mbarrier, and the ranking warps pick their keys up from there instead of issuing
 // IPT global loads each (B2_SORT_CFG=12; other tiles take the ordinary loads).
@@ -490,11 +637,7 @@ __global__ void __launch_bounds__(THREADS + 32 * LBW, MINB) onesweep_kernel(pass
 
   if (tid == 0) s_misc[0] = atomicAdd(a.tile_counter, 1u);
   if constexpr (BULK && !EMU_BUILD) {
-    if (tid == 0) {
-      const uint32_t mbar = (uint32_t)__cvta_generic_to_shared(s_misc + 12);  // 8-byte aligned slot behind the scan scratch (s_misc[1..8])
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(mbar) : "memory");
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) mbar_init_one((uint32_t)__cvta_generic_to_shared(s_misc + 12));  // 8-byte aligned slot behind the scan scratch (s_misc[1..8])
   }
   if (ranker) {
 #pragma unroll
@@ -606,16 +749,8 @@ __global__ void __launch_bounds__(THREADS + 32 * LBW, MINB) onesweep_kernel(pass
           ranker_barrier(THREADS);
         } else {
           const uint32_t mbar = (uint32_t)__cvta_generic_to_shared(s_misc + 12);
-          if (tid == 0) {
-            const uint32_t dst = (uint32_t)__cvta_generic_to_shared(s_keys);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(mbar), "r"(BYTES) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
-                         "l"(src + tile_base), "r"(BYTES), "r"(mbar)
-                         : "memory");
-          }
-          asm volatile(
-            "{\n .reg .pred p;\n BULK_WAIT:\n mbarrier.try_wait.parity.shared::cta.b64 p, [%0], 0;\n @p bra BULK_DONE;\n bra BULK_WAIT;\n BULK_DONE:\n}" ::"r"(mbar)
-            : "memory");
+          if (tid == 0) bulk_copy_to_smem(s_keys, src + tile_base, BYTES, mbar);
+          mbar_wait_phase0(mbar);
         }
 #pragma unroll
         for (int i = 0; i < IPT; ++i) key[i] = s_keys[warp * (32 * IPT) + i * 32 + lane];
@@ -671,14 +806,7 @@ __global__ void __launch_bounds__(THREADS + 32 * LBW, MINB) onesweep_kernel(pass
   };
   // ---- early counts: warp-private digit histogram by shared-memory atomics (no dependency chain) ----
   uint32_t* my_hist = s_whist + warp * RADIX;
-#pragma unroll
-  for (int i = 0; i < IPT; ++i) atomicAdd(&my_hist[digit_at(i)], 1u);
-  __syncwarp();
-  // number of distinct digits in this warp's 32*IPT keys: picks the ranking flavour below
-  int distinct = 0;
-#pragma unroll
-  for (int j = 0; j < RADIX / 32; ++j) distinct += my_hist[j * 32 + lane] != 0u;
-  distinct = __reduce_add_sync(0xffffffffu, distinct);
+  const int distinct = warp_digit_counts<IPT>(digit_at, IPT, lane, my_hist);
   ranker_barrier(THREADS);  // (S1)
 
   // ---- per digit: warp counts -> warp offsets; publish the aggregate ---------------------------
@@ -711,55 +839,9 @@ __global__ void __launch_bounds__(THREADS + 32 * LBW, MINB) onesweep_kernel(pass
   }
   cta_barrier(THREADS + 32 * LBW);  // (S2) releases the look-back warps; warp offsets final
 
-  // ---- rank within warp (stable): MATCH.ANY peers + running per-warp digit offsets --------------
-  // All MATCH ops are issued first (independent, pipelined); only the counter chain is serial.
-  // Peer masks (lanes of the warp holding the same digit; scripts/ubench/rank_probe.cu compares the strategies):
-  // MATCH.ANY is cheap only when the warp holds few distinct digits, the shared-memory atomicOr bitmap costs
-  // about the same at any digit mix.  Hence: bitmap for the general case, MATCH.ANY when the warp holds only a handful of distinct digits.
+  // ---- rank within warp (stable): peer masks + running per-warp digit offsets ---------------------
   uint32_t pos[IPT];
-  uint32_t* my_bm = s_bm + warp * RADIX;
-  if (distinct > 4) {
-#pragma unroll
-    for (int i = 0; i < IPT; ++i) {
-      const unsigned d = digit_at(i);
-      atomicOr(&my_bm[d], 1u << lane);
-      __syncwarp();
-      const unsigned peers = my_bm[d];
-      const unsigned lt = __popc(peers & lanemask_lt());
-      uint32_t prev = 0;
-      // The emulator (tests/emu) runs the lanes of a warp one after the other between rendezvous points, so the
-      // leader's clear below would be seen by the followers' read above. On the GPU the warp executes this
-      // straight-line stretch converged (validated on hardware); SAFE is the formally race-free variant.
-      if constexpr (SAFE || EMU_BUILD) __syncwarp();
-      if (lt == 0) {
-        if constexpr (RMW) {
-          prev = atomicAdd(&my_hist[d], (uint32_t)__popc(peers));
-        } else {
-          prev = my_hist[d];
-          my_hist[d] = prev + __popc(peers);
-        }
-        my_bm[d] = 0;
-      }
-      __syncwarp();
-      prev = __shfl_sync(0xffffffffu, prev, __ffs(peers) - 1);
-      pos[i] = prev + lt;
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < IPT; ++i) {
-      const unsigned d = digit_at(i);
-      const unsigned peers = __match_any_sync(0xffffffffu, d);
-      const unsigned lt = __popc(peers & lanemask_lt());
-      uint32_t prev = 0;
-      if (lt == 0) {
-        prev = my_hist[d];
-        my_hist[d] = prev + __popc(peers);
-      }
-      __syncwarp();
-      prev = __shfl_sync(0xffffffffu, prev, __ffs(peers) - 1);
-      pos[i] = prev + lt;
-    }
-  }
+  warp_rank<IPT, SAFE, RMW>(digit_at, IPT, distinct, lane, my_hist, s_bm + warp * RADIX, pos);
   // tile-sorted staging of the keys
 #pragma unroll
   for (int i = 0; i < IPT; ++i) s_keys[pos[i]] = key[i];
@@ -893,6 +975,58 @@ constexpr int FIX_IPT     = 8;
 constexpr int FIX_TILE    = FIX_THREADS * FIX_IPT;
 constexpr int FIX_HALO    = 64;
 
+// Walk of one row with key k over its segment (the neighbours whose keys agree with k on the bits >= shift): key_at(o) is
+// the key o rows away, lmax / rmax the rows that exist to the left / right (at most FIX_HALO). The row's final place is its
+// own minus `left` plus `before`; `cut`: a walk reached FIX_HALO rows, `all_equal`: every key it saw equals k.
+struct seg_walk {
+  int left, before;
+  bool all_equal, cut;
+};
+template <typename UK, int FIX_FAST, typename KeyAt>
+__device__ __forceinline__ seg_walk segment_walk(const KeyAt& key_at, UK k, int shift, int lmax, int rmax)
+{
+  const UK pf = k >> shift;
+  seg_walk w{0, 0, true, false};
+  // The first FIX_FAST neighbours on each side are examined without branches (every lane of the warp does the same
+  // work: a divergent walk costs the warp its LONGEST segment, which tripled the kernel's time at ~2 rows per segment);
+  // only rows whose segment reaches further continue with the loops below.
+  bool in_l = true, in_r = true;  // FIX_FAST = 0: no unrolled part, both walks start at the row itself
+#pragma unroll
+  for (int s = 1; s <= FIX_FAST; ++s) {
+    const UK ol = key_at(-s);   // inside the halo: FIX_HALO >= FIX_FAST
+    const UK orr = key_at(s);
+    in_l = in_l && s <= lmax && (UK)(ol >> shift) == pf;
+    in_r = in_r && s <= rmax && (UK)(orr >> shift) == pf;
+    w.left += in_l ? 1 : 0;
+    w.before += (in_l && ol <= k) ? 1 : 0;   // earlier rows win ties
+    w.before += (in_r && orr < k) ? 1 : 0;
+    w.all_equal = w.all_equal && (!in_l || ol == k) && (!in_r || orr == k);
+  }
+  int right = 0;
+  if (in_l) {  // the segment extends further to the left
+    for (;;) {
+      if (w.left == lmax) { w.cut = lmax == FIX_HALO; break; }
+      const UK o = key_at(-w.left - 1);
+      if ((UK)(o >> shift) != pf) break;
+      ++w.left;
+      w.before += o <= k ? 1 : 0;
+      w.all_equal = w.all_equal && o == k;
+    }
+  }
+  if (in_r) {
+    right = FIX_FAST;
+    for (;;) {
+      if (right == rmax) { w.cut = w.cut || rmax == FIX_HALO; break; }
+      const UK o = key_at(right + 1);
+      if ((UK)(o >> shift) != pf) break;
+      ++right;
+      w.before += o < k ? 1 : 0;
+      w.all_equal = w.all_equal && o == k;
+    }
+  }
+  return w;
+}
+
 template <typename UK, typename VT, int FIX_FAST>
 __global__ void __launch_bounds__(FIX_THREADS) segment_fix_kernel(pass_args a, int64_t n)
 {
@@ -921,57 +1055,188 @@ __global__ void __launch_bounds__(FIX_THREADS) segment_fix_kernel(pass_args a, i
       VT v{};
       if (a.pairs) v = ld_stream(vin + gi);
       const UK k  = sk[FIX_HALO + i];
-      const UK pf = k >> shift;
       // rows to the left / right that exist (array ends are segment ends)
       const int lmax = (int)(gi < FIX_HALO ? gi : (int64_t)FIX_HALO);
       const int rmax = (int)(n - 1 - gi < FIX_HALO ? n - 1 - gi : (int64_t)FIX_HALO);
-      int left = 0, before = 0;
-      bool all_equal = true, cut = false;
-      // The first FIX_FAST neighbours on each side are examined without branches (every lane of the warp does the same
-      // work: a divergent walk costs the warp its LONGEST segment, which tripled the kernel's time at ~2 rows per segment);
-      // only rows whose segment reaches further continue with the loops below.
-      bool in_l = true, in_r = true;  // FIX_FAST = 0: no unrolled part, both walks start at the row itself
-#pragma unroll
-      for (int s = 1; s <= FIX_FAST; ++s) {
-        const UK ol = sk[FIX_HALO + i - s];   // inside the halo: FIX_HALO >= FIX_FAST
-        const UK orr = sk[FIX_HALO + i + s];
-        in_l = in_l && s <= lmax && (UK)(ol >> shift) == pf;
-        in_r = in_r && s <= rmax && (UK)(orr >> shift) == pf;
-        left += in_l ? 1 : 0;
-        before += (in_l && ol <= k) ? 1 : 0;   // earlier rows win ties
-        before += (in_r && orr < k) ? 1 : 0;
-        all_equal = all_equal && (!in_l || ol == k) && (!in_r || orr == k);
-      }
-      int right = 0;
-      if (in_l) {  // the segment extends further to the left
-        for (;;) {
-          if (left == lmax) { cut = lmax == FIX_HALO; break; }
-          const UK o = sk[FIX_HALO + i - left - 1];
-          if ((UK)(o >> shift) != pf) break;
-          ++left;
-          before += o <= k ? 1 : 0;
-          all_equal = all_equal && o == k;
-        }
-      }
-      if (in_r) {
-        right = FIX_FAST;
-        for (;;) {
-          if (right == rmax) { cut = cut || rmax == FIX_HALO; break; }
-          const UK o = sk[FIX_HALO + i + right + 1];
-          if ((UK)(o >> shift) != pf) break;
-          ++right;
-          before += o < k ? 1 : 0;
-          all_equal = all_equal && o == k;
-        }
-      }
-      int64_t dst = gi - left + before;
-      if (cut) {
+      const seg_walk w = segment_walk<UK, FIX_FAST>([&](int o) { return sk[FIX_HALO + i + o]; }, k, shift, lmax, rmax);
+      int64_t dst = gi - w.left + w.before;
+      if (w.cut) {
         dst = gi;
-        if (!all_equal) atomicOr(&a.ctl->overflow, 1u);
+        if (!w.all_equal) atomicOr(&a.ctl->overflow, 1u);
       }
       if (a.pairs) vout[dst] = v;
       else kout[dst] = untwiddle_rt<UK>(k, a.kind, desc);
     }
+  }
+}
+
+// Range tier of the hybrid plan.  The executed LSD passes cover only the top digit(s) the range id is made of (the 16-bit
+// prefix for 1e9 uniform keys: ~15 K rows per range), so every range is a contiguous run of rows in input order.
+// range_sort_kernel sorts one range per CTA in shared memory: stable 8-bit ranking passes over the digits the hybrid plan
+// would have sorted below the prefix (ctl->range_digits), then the segment walk over the bits below ctl->fix_shift. This is
+// the order the hybrid plan's passes + segment_fix_kernel give, row for row: a range holds whole segments, and the walk keeps
+// FIX_HALO and the duplicate rule. A range longer than RANGE_CAP rows, or a cut walk over unequal keys, raises ctl->overflow
+// (the host reruns without the range tier).
+constexpr int RANGE_THREADS = 512;
+constexpr int RANGE_WARPS   = RANGE_THREADS / 32;
+constexpr int RANGE_IPT     = RANGE_CAP / RANGE_THREADS;  // local row ids fit 16 bits
+
+size_t range_sort_smem()
+{
+  // scratch (mbarrier, scan) + keys (one row of slack in front for the 16-byte aligned bulk copy) + per-warp counters and
+  // peer bitmaps + local row ids in sorted order
+  return 64 + sizeof(uint64_t) * (RANGE_CAP + 2) + sizeof(uint32_t) * 2 * RANGE_WARPS * RADIX + sizeof(uint16_t) * RANGE_CAP;
+}
+
+// bounds[i] = first row of range i in the keys the last executed pass wrote, bounds[nranges] = n. One thread per range: a
+// binary search over all rows (~30 dependent loads; the 65 537 searches run in parallel).
+__global__ void range_bounds_kernel(pass_args a, int64_t n, uint32_t* __restrict__ bounds, int nranges)
+{
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i > nranges) return;
+  const uint64_t* __restrict__ keys = static_cast<const uint64_t*>(a.ctl->fix_key_buf == 1 ? a.key_bufs[1] : a.key_bufs[2]);
+  const int sh = a.ctl->range_shift;
+  const uint64_t mask = (uint64_t)nranges - 1;
+  int64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const int64_t mid = (lo + hi) >> 1;
+    if ((int64_t)((keys[mid] >> sh) & mask) < i) lo = mid + 1;
+    else hi = mid;
+  }
+  bounds[i] = (uint32_t)lo;
+}
+
+template <typename VT>
+__global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
+{
+  using UK = uint64_t;
+  B2_DYNAMIC_SMEM(smem_raw);
+  uint32_t* s_misc  = reinterpret_cast<uint32_t*>(smem_raw);                       // [0..1] mbarrier, [8..15] digit scan
+  UK* s_keys        = reinterpret_cast<UK*>(smem_raw + 64);                        // [RANGE_CAP + 2]
+  uint32_t* s_whist = reinterpret_cast<uint32_t*>(s_keys + RANGE_CAP + 2);        // [RANGE_WARPS][256]
+  uint32_t* s_bm    = s_whist + RANGE_WARPS * RADIX;                               // [RANGE_WARPS][256]
+  uint16_t* s_perm  = reinterpret_cast<uint16_t*>(s_bm + RANGE_WARPS * RADIX);    // [RANGE_CAP] local row of sorted position
+
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t s = bounds[blockIdx.x];
+  const int m = (int)(bounds[blockIdx.x + 1] - s);
+  if (m == 0) return;
+  if (m > RANGE_CAP) {
+    if (tid == 0) atomicOr(&a.ctl->overflow, 1u);
+    return;
+  }
+  const UK* __restrict__ keys = static_cast<const UK*>(a.ctl->fix_key_buf == 1 ? a.key_bufs[1] : a.key_bufs[2]) + s;
+  const VT* __restrict__ vin  = reinterpret_cast<const VT*>(a.ctl->fix_idx_buf == 1 ? a.idx_bufs[1] : a.idx_bufs[2]) + s;
+  VT* __restrict__ vout = reinterpret_cast<VT*>(a.idx_bufs[0]) + s;
+  UK* __restrict__ kout = static_cast<UK*>(const_cast<void*>(a.key_bufs[1])) + s;
+
+  // ---- keys -> s_keys[off + r]: the 16-byte aligned rows [-off, 2 * ((m + off) / 2) - off) by one bulk copy, an odd last row
+  // by an ordinary load (the emulator replays the bulk copy with ordinary loads)
+  const int off = (int)((reinterpret_cast<uintptr_t>(keys) & 15) / sizeof(UK));
+  const bool bulk = (reinterpret_cast<uintptr_t>(keys) & 7) == 0 && s >= off && m + off >= 2;
+  const int bulk_rows = bulk ? (m + off) / 2 * 2 : 0;
+  const uint32_t mbar = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc);
+  if constexpr (!EMU_BUILD) {
+    if (tid == 0 && bulk) mbar_init_one(mbar);
+  }
+#pragma unroll
+  for (int j = 0; j < RADIX / 32; ++j) s_bm[warp * RADIX + j * 32 + lane] = 0;
+  __syncthreads();
+  const int base = bulk ? off : 0;
+  if (bulk) {
+    if constexpr (EMU_BUILD) {
+      for (int q = tid; q < bulk_rows; q += RANGE_THREADS) s_keys[q] = keys[q - off];
+    } else {
+      if (tid == 0) {
+        bulk_copy_to_smem(s_keys, keys - off, (uint32_t)(sizeof(UK) * bulk_rows), mbar);
+        // the payload window is read in sorted order at the end: bring it into L2 while the keys are ranked
+        if (a.pairs) {
+          const uintptr_t lo = reinterpret_cast<uintptr_t>(vin) & ~uintptr_t(15);
+          const uintptr_t hi = (reinterpret_cast<uintptr_t>(vin + m) + 15) & ~uintptr_t(15);
+          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((uint32_t)(hi - lo)) : "memory");
+        }
+      }
+    }
+    if (tid == 0 && bulk_rows - off < m) s_keys[base + m - 1] = keys[m - 1];
+  } else {
+    for (int q = tid; q < m; q += RANGE_THREADS) s_keys[q] = ld_stream(keys + q);
+  }
+  if constexpr (!EMU_BUILD) {
+    if (bulk) mbar_wait_phase0(mbar);
+  }
+  __syncthreads();
+
+  // ---- stable LSD ranking passes over the range's remaining digits, lowest first; s_perm[pos] = local row --------------
+  // item i of lane l in warp w is position w * 32 * nit + 32 * i + l of the previous order; positions >= m are padding with
+  // digit 255, which the stable ranking puts behind every row
+  const int nit = (m + RANGE_THREADS - 1) / RANGE_THREADS;
+  const int wbase = warp * 32 * nit + lane;
+  uint32_t* my_hist = s_whist + warp * RADIX;
+  bool first = true;
+  for (uint32_t digits = a.ctl->range_digits; digits != 0; digits &= digits - 1) {
+    const int sh = 8 * (__ffs(digits) - 1);
+    uint32_t pk[RANGE_IPT];  // local row | digit << 16
+#pragma unroll
+    for (int i = 0; i < RANGE_IPT; ++i) {
+      if (i >= nit) break;
+      const int q = wbase + 32 * i;
+      const uint32_t r = q < m ? (first ? (uint32_t)q : (uint32_t)s_perm[q]) : 0u;
+      const uint32_t dg = q < m ? (uint32_t)(s_keys[base + r] >> sh) & 255u : 255u;
+      pk[i] = r | dg << 16;
+    }
+#pragma unroll
+    for (int j = 0; j < RADIX / 32; ++j) my_hist[j * 32 + lane] = 0;
+    __syncwarp();
+    auto digit_at = [&](int i) -> unsigned { return pk[i] >> 16; };
+    const int distinct = warp_digit_counts<RANGE_IPT>(digit_at, nit, lane, my_hist);
+    __syncthreads();
+    // digit d of warp w starts at (rows of digits < d) + (rows of digit d in warps < w)
+    uint32_t cnt = 0, inc = 0;
+    if (tid < RADIX) {
+#pragma unroll
+      for (int w = 0; w < RANGE_WARPS; ++w) {
+        const uint32_t c = s_whist[w * RADIX + tid];
+        s_whist[w * RADIX + tid] = cnt;
+        cnt += c;
+      }
+      inc = warp_inclusive_sum(cnt);
+      if (lane == 31) s_misc[8 + warp] = inc;
+    }
+    __syncthreads();
+    if (tid < RADIX) {
+      uint32_t start = inc - cnt;
+      for (int w = 0; w < warp; ++w) start += s_misc[8 + w];
+#pragma unroll
+      for (int w = 0; w < RANGE_WARPS; ++w) s_whist[w * RADIX + tid] += start;
+    }
+    __syncthreads();
+    uint32_t pos[RANGE_IPT];
+    warp_rank<RANGE_IPT, true, true>(digit_at, nit, distinct, lane, my_hist, s_bm + warp * RADIX, pos);
+#pragma unroll
+    for (int i = 0; i < RANGE_IPT; ++i) {
+      if (i >= nit) break;
+      if (wbase + 32 * i < m) s_perm[pos[i]] = (uint16_t)(pk[i] & 0xffffu);
+    }
+    __syncthreads();
+    first = false;
+  }
+
+  // ---- segment walk over the bits below fix_shift; a range edge is a segment edge ----------------------------------------
+  const int shift = a.ctl->fix_shift;
+  const UK desc = (UK)a.desc_mask;
+  for (int r = tid; r < m; r += RANGE_THREADS) {
+    const int lr = s_perm[r];
+    const UK k = s_keys[base + lr];
+    const int lmax = min(r, FIX_HALO);
+    const int rmax = min(m - 1 - r, FIX_HALO);
+    const seg_walk w = segment_walk<UK, 0>([&](int o) { return s_keys[base + s_perm[r + o]]; }, k, shift, lmax, rmax);
+    int dst = r - w.left + w.before;
+    if (w.cut) {
+      dst = r;
+      if (!w.all_equal) atomicOr(&a.ctl->overflow, 1u);
+    }
+    if (a.pairs) vout[dst] = vin[lr];
+    else kout[dst] = untwiddle_rt<UK>(k, a.kind, desc);
   }
 }
 
@@ -1121,6 +1386,18 @@ int64_t portion_limit()
 
 // B2_SORT_HYBRID=0 switches the partial-LSD + fix-up plan off; B2_SORT_HYBRID_MIN=<rows> moves its lower size limit
 // (tests run it on small inputs).
+// range tier of the hybrid plan: from this size on by default (measured on the H100: DESIGN.md §4.1); B2_SORT_RANGE=0 / 1
+// (test hook) forces it off / on wherever the plan finds it feasible
+constexpr int64_t RANGE_MIN_ROWS = int64_t(1) << 27;
+int range_env()
+{
+  static int v = [] {
+    const char* e = std::getenv("B2_SORT_RANGE");
+    return e ? (std::atoi(e) != 0 ? 1 : 0) : -1;
+  }();
+  return v;
+}
+
 int64_t hybrid_min_rows()
 {
   static int64_t v = [] {
@@ -1167,11 +1444,17 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
   once_per_device(attr_done, [] {
     B2_CUDA_TRY(cudaFuncSetAttribute(onesweep_kernel<UK, T, I, MINB, VT, CARRY, MIX, SAFE, RMW, BULK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      (int)onesweep_smem<UK, T, I, VT>()));
+    if constexpr (sizeof(UK) == 8 && !MIX)
+      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem()));
   });
 
   // Hybrid plan (64-bit raw keys, full sort): LSD passes over the top digits only, then segment_fix_kernel. The plan
   // kernel decides on the device; the host learns the outcome from one 4-byte read-back after the fix-up.
   bool try_hybrid = sizeof(UK) == 8 && !MIX && raw && first_pass == 0 && last_pass >= NP - 1 && !keep_keys && n >= hybrid_min_rows();
+  // Its range tier (range_sort_kernel) from RANGE_MIN_ROWS rows on; B2_SORT_RANGE=0 / 1 (test hook) switches it off / on at
+  // any size. The host reads the plan back to size the range launches.
+  const int force_range = range_env();
+  bool try_range = try_hybrid && force_range != 0 && (force_range == 1 || n >= RANGE_MIN_ROWS);
 
   for (;;) {
     // control block, histograms and tile counters are zeroed here; the look-back rows of a (pass, portion) right before its launch, so
@@ -1191,13 +1474,15 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
           B2_LAUNCH((histogram_kernel<UK, MIX>), grid, 512, 0, stream, hkeys, n, raw ? 1 : 0, kind, desc_mask, ghist, nanp, 0xf0u,
                     (const int32_t*)nullptr, &ctl->vary);
         }
-        B2_LAUNCH(plan_kernel, 1, RADIX, 0, stream, ghist, NP, (uint32_t)n, raw ? 1 : 0, pre_idx_buf, ctl, first_pass, last_pass, 1, 1);
+        B2_LAUNCH(plan_kernel, 1, RADIX, 0, stream, ghist, NP, (uint32_t)n, raw ? 1 : 0, pre_idx_buf, ctl, first_pass, last_pass, 1, 1,
+                  try_range ? 1 : 0);
         {
           prof_scope ps("histogram", stream);
           B2_LAUNCH((histogram_kernel<UK, MIX>), grid, 512, 0, stream, hkeys, n, raw ? 1 : 0, kind, desc_mask, ghist, (uint32_t*)nullptr, 0x0fu,
                     &ctl->need_low, (unsigned long long*)nullptr);
         }
-        B2_LAUNCH(plan_kernel, 1, RADIX, 0, stream, ghist, NP, (uint32_t)n, raw ? 1 : 0, pre_idx_buf, ctl, first_pass, last_pass, 1, 2);
+        B2_LAUNCH(plan_kernel, 1, RADIX, 0, stream, ghist, NP, (uint32_t)n, raw ? 1 : 0, pre_idx_buf, ctl, first_pass, last_pass, 1, 2,
+                  try_range ? 1 : 0);
       } else {
         {
           prof_scope ps("histogram", stream);
@@ -1233,19 +1518,22 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
     // Small inputs launch every digit's kernel and stay free of host synchronisation.
     uint32_t skip_mask = 0;
     bool plan_hybrid = true;
+    int range_bits = 0;  // range tier: the range id has range_bits bits
     static const int64_t readback_min = [] {
       const char* e = std::getenv("B2_SORT_PLAN_READBACK_MIN");  // test hook
       return e ? (int64_t)std::atoll(e) : (int64_t(1) << 22);
     }();
-    if (n >= readback_min) {
+    if (n >= readback_min || try_range) {
       pass_plan hp[8];
-      int32_t hflag = 0;
+      int32_t hflag = 0, hrange[3] = {0, 0, 0};  // ctl->range, range_shift, range_bits
       B2_CUDA_TRY(cudaMemcpyAsync(hp, &ctl->plan[0], sizeof(pass_plan) * 8, cudaMemcpyDeviceToHost, stream));
       B2_CUDA_TRY(cudaMemcpyAsync(&hflag, &ctl->hybrid, sizeof(int32_t), cudaMemcpyDeviceToHost, stream));
+      if (try_range) B2_CUDA_TRY(cudaMemcpyAsync(hrange, &ctl->range, sizeof(hrange), cudaMemcpyDeviceToHost, stream));
       B2_CUDA_TRY(cudaStreamSynchronize(stream));
       for (int p = 0; p < NP; ++p)
         if (hp[p].trivial) skip_mask |= 1u << p;
       plan_hybrid = hflag != 0;
+      range_bits = hrange[0] ? hrange[2] : 0;
     }
     for (int p = std::max(0, first_pass); p < NP && p <= last_pass; ++p) {
       if ((skip_mask >> p) & 1u) continue;
@@ -1267,7 +1555,16 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
       }
     }
     if constexpr (sizeof(UK) == 8 && !MIX) {
-      if (try_hybrid && plan_hybrid) {
+      if (try_hybrid && plan_hybrid && range_bits) {
+        const int nranges = 1 << range_bits;
+        dbuf bounds(sizeof(uint32_t) * (nranges + 1), stream);
+        {
+          prof_scope ps("range_bounds", stream);
+          B2_LAUNCH(range_bounds_kernel, (nranges + 256) / 256, 256, 0, stream, a, n, bounds.as<uint32_t>(), nranges);
+        }
+        prof_scope ps("segment_fix", stream);  // the range sort replaces the segment fix-up
+        B2_LAUNCH((range_sort_kernel<VT>), nranges, RANGE_THREADS, range_sort_smem(), stream, a, bounds.as<const uint32_t>());
+      } else if (try_hybrid && plan_hybrid) {
         const int64_t ntiles = (n + FIX_TILE - 1) / FIX_TILE;
         const int grid = (int)std::min<int64_t>(ntiles, num_sms() * 8);
         prof_scope ps("segment_fix", stream);
@@ -1284,6 +1581,10 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
     B2_CUDA_TRY(cudaMemcpyAsync(&overflow, &ctl->overflow, sizeof(overflow), cudaMemcpyDeviceToHost, stream));
     B2_CUDA_TRY(cudaStreamSynchronize(stream));
     if (!overflow) break;
+    if (range_bits) {  // a range did not fit (or held unequal keys beyond the walk window): the hybrid plan without the range tier
+      try_range = false;
+      continue;
+    }
     try_hybrid = false;  // a segment was longer than the fix-up window (digits not independent): full LSD sort of the untouched input
   }
   if (pairs && raw && kind == (int)key_kind::FLOAT && descending) {

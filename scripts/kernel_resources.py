@@ -46,9 +46,10 @@ for line in sass.splitlines():
                 mnem[cur][key] = mnem[cur].get(key, 0) + 1
 print("# Static resources of the shipped kernels (sm_90a; `scripts/kernel_resources.py`, no GPU involved)\n")
 print("Registers / stack / static shared memory from `cuobjdump --dump-resource-usage cudf_b200/libcudf_b200.so`; dynamic shared memory is set at")
-print("launch (one-sweep (key, 8-byte payload): 76.9 KB -> two CTAs of 448 threads per SM; `rj_join_kernel`: 160 KB, one CTA of 1024; `pgb_agg_kernel`:")
-print("160 KB, one CTA of 1024). Mnemonic counts are static occurrences in the SASS (UBLKCP = `cp.async.bulk`, the 1-D TMA path, only in the")
-print("`B2_SORT_CFG=12` instantiation; SYNCS = mbarrier operations).\n")
+print("launch (one-sweep with 8-byte keys: 76.9 KB at 384 x 16 -> two CTAs of 448 threads per SM, 117.8 KB at 512 x 20 -> one CTA of 576;")
+print("`rj_join_kernel`: 160 KB, one CTA of 1024; `pgb_agg_kernel`: 160 KB, one CTA of 1024). Mnemonic counts are static occurrences in the")
+print("SASS (UBLKCP = `cp.async.bulk`, the 1-D TMA path, only in the 512 x 20 payload-carrying one-sweep instantiation and in")
+print("`range_sort_kernel`; SYNCS = mbarrier operations).\n")
 print("| Kernel | regs | stack | static smem | SASS mnemonics (static count) |")
 print("|---|---|---|---|---|")
 for name, reg, stack, sh in sorted(rows, key=lambda r: dm[r[0]]):

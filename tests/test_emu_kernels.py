@@ -42,7 +42,7 @@ def emu_lib():
 
 def run(code: str, marker: str, env=None, timeout=900):
     e = dict(os.environ)
-    for k in ("B2_JOIN_RADIX_CAPACITY", "B2_SORT_PLAN_READBACK_MIN", "B2_GROUPBY_PARTITION_ROWS", "B2_GROUPBY_SMEM_SLOTS", "B2_SORT_HYBRID", "B2_SORT_HYBRID_MIN", "B2_SORT_FIX_FAST", "B2_SORT_CARRY", "B2_SORT_ALIAS", "B2_JOIN_RADIX_ROWS", "B2_JOIN_KERNEL", "B2_GROUPBY_EST", "B2_GROUPBY_EST_MIN", "B2_GROUPBY_EST_CAP", "B2_JOIN_PARTITION_ROWS", "B2_SORT_CFG", "B2_SORT_PORTION"):
+    for k in ("B2_JOIN_RADIX_CAPACITY", "B2_SORT_PLAN_READBACK_MIN", "B2_GROUPBY_PARTITION_ROWS", "B2_GROUPBY_SMEM_SLOTS", "B2_SORT_HYBRID", "B2_SORT_HYBRID_MIN", "B2_SORT_FIX_FAST", "B2_SORT_CARRY", "B2_SORT_ALIAS", "B2_JOIN_RADIX_ROWS", "B2_JOIN_KERNEL", "B2_GROUPBY_EST", "B2_GROUPBY_EST_MIN", "B2_GROUPBY_EST_CAP", "B2_JOIN_PARTITION_ROWS", "B2_SORT_PORTION"):
         e.pop(k, None)
     e.update(env or {})
     r = subprocess.run([sys.executable, "-c", PRELUDE + code], capture_output=True, text=True, env=e, cwd=ROOT, timeout=timeout)
@@ -95,13 +95,6 @@ offs = np.sort(rng.integers(0, 70_000, 300)).astype(np.int32); offs[0] = 0
 assert_columns_equal(cu.segmented_reduce(x, offs, "sum", np.int64), o.segmented_reduce(x, offs, "sum", np.int64), what="segmented")
 print('VALIDATED_OK')
 """, "VALIDATED_OK", env={"B2_SORT_PORTION": "12288"})
-
-
-@pytest.mark.parametrize("cfg", ["3", "10", "11", "12"])
-def test_emu_sort_tile_variants(emu_lib, cfg):
-    """B2_SORT_CFG variants of the 64-bit one-sweep kernel (another tile shape, the race-free and the ATOMS.ADD ranking, the
-    bulk-copy key load — whose data movement the emulator replays with ordinary loads)."""
-    run(SORT_PAYLOAD, "SORT_PAYLOAD_OK", env={"B2_SORT_CFG": cfg})
 
 
 def test_emu_sort_carry_payload(emu_lib):

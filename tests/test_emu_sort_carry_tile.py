@@ -1,9 +1,7 @@
-"""The payload-carrying 64-bit sort_by_key pass on the CPU emulator: the default for 8-byte payloads (512 x 20 tiles, one CTA
-per SM, key tiles by one bulk async copy, which the emulator replays with ordinary loads) and B2_SORT_CFG=13, the 384 x 16
-tile with two CTAs per SM that 4-byte payloads keep."""
-import pytest
-
-from tests.test_emu_kernels import SORT_PAYLOAD, emu_lib, run  # noqa: F401  (emu_lib is a fixture)
+"""The payload-carrying 64-bit sort_by_key pass on the CPU emulator: 8-byte payloads take 512 x 20 tiles, one CTA per SM, key
+tiles by one bulk async copy (which the emulator replays with ordinary loads); 4-byte payloads keep the 384 x 16 tile with two
+CTAs per SM (the SLICED cases include one)."""
+from tests.test_emu_kernels import emu_lib, run  # noqa: F401  (emu_lib is a fixture)
 
 TILE = 512 * 20
 
@@ -39,13 +37,8 @@ print('PORTIONS_OK')
 """
 
 
-def test_emu_sort_carry_previous_tile(emu_lib):
-    run(SORT_PAYLOAD, "SORT_PAYLOAD_OK", env={"B2_SORT_CFG": "13"})
-
-
-@pytest.mark.parametrize("cfg", ["0", "13"])
-def test_emu_sort_carry_sliced(emu_lib, cfg):
-    run(f"TILE = {TILE}\n" + SLICED, "SLICED_OK", env={"B2_SORT_CFG": cfg})
+def test_emu_sort_carry_sliced(emu_lib):
+    run(f"TILE = {TILE}\n" + SLICED, "SLICED_OK")
 
 
 def test_emu_sort_carry_portions(emu_lib):

@@ -66,11 +66,10 @@ struct sort_ctl {
   int32_t fix_fast;            // hybrid plan: which segment_fix_kernel instantiation runs (0: plain walks, 1: branch-free first neighbours)
   unsigned long long vary;     // OR of (key ^ first key) over the input
   // range tier of the hybrid plan (see range_sort_kernel): the executed passes sort only the range id = (key >> range_shift) &
-  // (2^range_bits - 1); each range is then sorted in shared memory by the digits in range_digits and the segment walk
+  // (2^range_bits - 1); each range is then sorted in shared memory by the bits below range_shift
   int32_t range;
   int32_t range_shift;
   int32_t range_bits;
-  uint32_t range_digits;       // bit p: digit p is ranked inside the ranges
 };
 
 template <typename UK>
@@ -246,7 +245,7 @@ constexpr int HYB_MIN_SAVED_PASSES = 2;
 // at once when phase 1 was final).
 // range_allowed (hybrid plan only): the caller can run range_sort_kernel. The plan then stops the passes at the top one or two
 // adjacent non-trivial digits once the expected range, n * prod coll, stays below RANGE_CAP by five standard deviations of a
-// uniform spread (1e9 uniform keys: 15 259 + 5 * 124 rows against 16 384), and at least one digit is left to rank in the ranges.
+// uniform spread (1e9 uniform keys: 15 259 + 5 * 124 rows against 16 384), and at least one digit is left to sort inside the ranges.
 constexpr int RANGE_CAP = 16384;  // rows of one range: range_sort_kernel holds its keys in 128 KB of shared memory
 __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint32_t n, int raw, int pre_idx_buf,
                             sort_ctl* ctl, int first_pass, int last_pass, int hyb_allowed, int phase = 0, int range_allowed = 0)
@@ -317,7 +316,6 @@ __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint3
       ctl->need_low = 0;
     }
     int range = 0, range_low = 0, range_bits = 0;
-    uint32_t range_digits = 0;
     if (hybrid && range_allowed) {
       double e = (double)n;
       for (int p = npass - 1; p > low && range_bits < 16; --p) {
@@ -328,8 +326,7 @@ __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint3
         e *= coll[p];
         range_bits += RADIX_BITS;
         if (e + 5.0 * sqrt(e) <= (double)RANGE_CAP) {
-          for (int q = low; q < p; ++q) range_digits |= triv[q] ? 0u : 1u << q;
-          range = range_digits != 0;
+          for (int q = low; q < p; ++q) range = range || !triv[q];  // at least one digit left to sort inside the ranges
           range_low = p;
           break;
         }
@@ -343,7 +340,6 @@ __global__ void plan_kernel(const uint32_t* __restrict__ ghist, int npass, uint3
     ctl->range        = range;
     ctl->range_shift  = range_low * RADIX_BITS;
     ctl->range_bits   = range ? range_bits : 0;
-    ctl->range_digits = range_digits;
     ctl->hybrid    = hybrid;
     // expected rows per segment decides the fix-up flavour: mostly single-row segments (1e9 uniform keys: 0.23) take the
     // plain walks, ~2-row segments (a rank's shard of the sharded sort: 1.9) the branch-free form
@@ -1073,21 +1069,29 @@ __global__ void __launch_bounds__(FIX_THREADS) segment_fix_kernel(pass_args a, i
 }
 
 // Range tier of the hybrid plan.  The executed LSD passes cover only the top digit(s) the range id is made of (the 16-bit
-// prefix for 1e9 uniform keys: ~15 K rows per range), so every range is a contiguous run of rows in input order.
-// range_sort_kernel sorts one range per CTA in shared memory: stable 8-bit ranking passes over the digits the hybrid plan
-// would have sorted below the prefix (ctl->range_digits), then the segment walk over the bits below ctl->fix_shift. This is
-// the order the hybrid plan's passes + segment_fix_kernel give, row for row: a range holds whole segments, and the walk keeps
-// FIX_HALO and the duplicate rule. A range longer than RANGE_CAP rows, or a cut walk over unequal keys, raises ctl->overflow
-// (the host reruns without the range tier).
-constexpr int RANGE_THREADS = 512;
-constexpr int RANGE_WARPS   = RANGE_THREADS / 32;
-constexpr int RANGE_IPT     = RANGE_CAP / RANGE_THREADS;  // local row ids fit 16 bits
+// prefix for 1e9 uniform keys: ~15 K rows per range), so every range is a contiguous run of rows in input order and its keys
+// agree on every bit at and above ctl->range_shift.  range_sort_kernel sorts one range per CTA in shared memory:
+//   1. bucket: the next bits below the range id that vary over the input (ctl->vary), up to 2^RANGE_BUCKET_BITS buckets
+//      (~2 rows per bucket at RANGE_CAP rows), so the bucket is monotone in the key; one shared-memory counting pass
+//      (histogram, scan, unstable scatter of the local rows) groups the range by bucket;
+//   2. order each bucket directly: a row's place is its bucket's start + the number of the bucket's rows with a smaller
+//      (key, local row), so equal keys keep their input order: the stable sort, the hybrid plan's order row for row;
+//   3. write: the payload window (in L2 from a prefetch issued with the key load) replaces the dead keys in shared memory
+//      by a second bulk copy, and every output row is written coalesced from there.
+// A range longer than RANGE_CAP rows, or a bucket longer than RANGE_BUCKET_CAP rows (many equal or clustered keys), raises
+// ctl->overflow (the host reruns without the range tier).
+constexpr int RANGE_THREADS     = 512;
+constexpr int RANGE_WARPS       = RANGE_THREADS / 32;
+constexpr int RANGE_IPT         = RANGE_CAP / RANGE_THREADS;  // local row ids fit 16 bits
+constexpr int RANGE_BUCKET_BITS = 13;
+constexpr int RANGE_BUCKETS     = 1 << RANGE_BUCKET_BITS;
+constexpr int RANGE_BUCKET_CAP  = FIX_HALO;  // rows of one bucket: each row compares its key with all of them
 
 size_t range_sort_smem()
 {
-  // scratch (mbarrier, scan) + keys (one row of slack in front for the 16-byte aligned bulk copy) + per-warp counters and
-  // peer bitmaps + local row ids in sorted order
-  return 64 + sizeof(uint64_t) * (RANGE_CAP + 2) + sizeof(uint32_t) * 2 * RANGE_WARPS * RADIX + sizeof(uint16_t) * RANGE_CAP;
+  // scratch (mbarriers, overflow flag, scan) + keys, later the payload (one row of slack in front for the 16-byte aligned bulk
+  // copy) + bucket counters + local row ids grouped by bucket, then in sorted order
+  return 128 + sizeof(uint64_t) * (RANGE_CAP + 2) + sizeof(uint32_t) * RANGE_BUCKETS + sizeof(uint16_t) * RANGE_CAP;
 }
 
 // bounds[i] = first row of range i in the keys the last executed pass wrote, bounds[nranges] = n. One thread per range: a
@@ -1108,16 +1112,44 @@ __global__ void range_bounds_kernel(pass_args a, int64_t n, uint32_t* __restrict
   bounds[i] = (uint32_t)lo;
 }
 
+// Rows [0, m) of the window g (row s of its buffer) -> sdst[base + r]; returns base. The 16-byte aligned rows
+// [-base, (m + base) / PER * PER - base) come by one bulk copy completing on `mbar` (the caller waits when `bulk`), the rows
+// behind them by ordinary loads; a misaligned window, or one whose aligned start would lie before its buffer, takes ordinary
+// loads only. The emulator replays the bulk copy with ordinary loads.
+struct range_window {
+  int base;
+  bool bulk;
+};
+template <typename T>
+__device__ __forceinline__ range_window range_window_load(T* sdst, const T* __restrict__ g, int64_t s, int m, uint32_t mbar)
+{
+  constexpr int PER = 16 / sizeof(T);
+  const int off  = (int)((reinterpret_cast<uintptr_t>(g) & 15) / sizeof(T));
+  const bool bulk = (reinterpret_cast<uintptr_t>(g) % sizeof(T)) == 0 && s >= off && m + off >= PER;
+  const int bulk_rows = bulk ? (m + off) / PER * PER : 0;
+  if (bulk) {
+    if constexpr (EMU_BUILD) {
+      for (int q = threadIdx.x; q < bulk_rows; q += RANGE_THREADS) sdst[q] = g[q - off];
+    } else {
+      if (threadIdx.x == 0) bulk_copy_to_smem(sdst, g - off, (uint32_t)(sizeof(T) * bulk_rows), mbar);
+    }
+    for (int r = bulk_rows - off + (int)threadIdx.x; r < m; r += RANGE_THREADS) sdst[off + r] = g[r];
+  } else {
+    for (int q = threadIdx.x; q < m; q += RANGE_THREADS) sdst[q] = ld_stream(g + q);
+  }
+  return {bulk ? off : 0, bulk};
+}
+
 template <typename VT>
 __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
 {
   using UK = uint64_t;
   B2_DYNAMIC_SMEM(smem_raw);
-  uint32_t* s_misc  = reinterpret_cast<uint32_t*>(smem_raw);                       // [0..1] mbarrier, [8..15] digit scan
-  UK* s_keys        = reinterpret_cast<UK*>(smem_raw + 64);                        // [RANGE_CAP + 2]
-  uint32_t* s_whist = reinterpret_cast<uint32_t*>(s_keys + RANGE_CAP + 2);        // [RANGE_WARPS][256]
-  uint32_t* s_bm    = s_whist + RANGE_WARPS * RADIX;                               // [RANGE_WARPS][256]
-  uint16_t* s_perm  = reinterpret_cast<uint16_t*>(s_bm + RANGE_WARPS * RADIX);    // [RANGE_CAP] local row of sorted position
+  uint32_t* s_misc = reinterpret_cast<uint32_t*>(smem_raw);                 // [0..1] / [2..3] key / payload mbarrier, [4] overflow, [16..31] scan
+  UK* s_keys       = reinterpret_cast<UK*>(smem_raw + 128);                  // [RANGE_CAP + 2]
+  VT* s_vals       = reinterpret_cast<VT*>(s_keys);                          // the payload window once the keys are dead
+  uint32_t* s_cnt  = reinterpret_cast<uint32_t*>(s_keys + RANGE_CAP + 2);   // [RANGE_BUCKETS] bucket counters
+  uint16_t* s_perm = reinterpret_cast<uint16_t*>(s_cnt + RANGE_BUCKETS);    // [RANGE_CAP] local rows by bucket, then sorted
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t s = bounds[blockIdx.x];
@@ -1132,113 +1164,119 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   VT* __restrict__ vout = reinterpret_cast<VT*>(a.idx_bufs[0]) + s;
   UK* __restrict__ kout = static_cast<UK*>(const_cast<void*>(a.key_bufs[1])) + s;
 
-  // ---- keys -> s_keys[off + r]: the 16-byte aligned rows [-off, 2 * ((m + off) / 2) - off) by one bulk copy, an odd last row
-  // by an ordinary load (the emulator replays the bulk copy with ordinary loads)
-  const int off = (int)((reinterpret_cast<uintptr_t>(keys) & 15) / sizeof(UK));
-  const bool bulk = (reinterpret_cast<uintptr_t>(keys) & 7) == 0 && s >= off && m + off >= 2;
-  const int bulk_rows = bulk ? (m + off) / 2 * 2 : 0;
-  const uint32_t mbar = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc);
+  // bucket = the nb bits below the highest bit under the range id that varies over the input (bits between it and the range id
+  // are the same in every key); nb ~ log2 m, at most RANGE_BUCKET_BITS. Counter of bucket b: slot (b mod per) * RANGE_THREADS +
+  // b / per, so that thread t scans the `per` consecutive buckets t * per + j at conflict-free slots j * RANGE_THREADS + t.
+  const uint64_t below = a.ctl->vary & ((1ull << a.ctl->range_shift) - 1);
+  const uint32_t vhi = (uint32_t)(below >> 32), vlo = (uint32_t)below;
+  const int top = vhi ? 64 - __clz((int)vhi) : (vlo ? 32 - __clz((int)vlo) : 0);  // bits [0, top) may differ within a range
+  const int want = m > 1 ? 32 - __clz(m - 1) : 0;                                     // ceil(log2 m)
+  const int nb = min(min(want, RANGE_BUCKET_BITS), top);
+  const int bshift = top - nb;
+  const uint32_t bmask = (1u << nb) - 1;
+  const int lp = max(nb - 9, 0);  // log2 per; RANGE_THREADS = 2^9
+  const int per = 1 << lp;
+  auto bucket = [&](UK k) { return (uint32_t)(k >> bshift) & bmask; };
+  auto slot   = [&](uint32_t b) { return ((b & (uint32_t)(per - 1)) << 9) | (b >> lp); };
+
+  const uint32_t mbar_k = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc);
+  const uint32_t mbar_v = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc + 2);
   if constexpr (!EMU_BUILD) {
-    if (tid == 0 && bulk) mbar_init_one(mbar);
-  }
-#pragma unroll
-  for (int j = 0; j < RADIX / 32; ++j) s_bm[warp * RADIX + j * 32 + lane] = 0;
-  __syncthreads();
-  const int base = bulk ? off : 0;
-  if (bulk) {
-    if constexpr (EMU_BUILD) {
-      for (int q = tid; q < bulk_rows; q += RANGE_THREADS) s_keys[q] = keys[q - off];
-    } else {
-      if (tid == 0) {
-        bulk_copy_to_smem(s_keys, keys - off, (uint32_t)(sizeof(UK) * bulk_rows), mbar);
-        // the payload window is read in sorted order at the end: bring it into L2 while the keys are ranked
-        if (a.pairs) {
-          const uintptr_t lo = reinterpret_cast<uintptr_t>(vin) & ~uintptr_t(15);
-          const uintptr_t hi = (reinterpret_cast<uintptr_t>(vin + m) + 15) & ~uintptr_t(15);
-          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((uint32_t)(hi - lo)) : "memory");
-        }
-      }
+    if (tid == 0) {
+      mbar_init_one(mbar_k);
+      mbar_init_one(mbar_v);
     }
-    if (tid == 0 && bulk_rows - off < m) s_keys[base + m - 1] = keys[m - 1];
+  }
+  if (tid == 0) s_misc[4] = 0;
+  for (int i = tid; i <= (int)bmask; i += RANGE_THREADS) s_cnt[i] = 0;
+  __syncthreads();
+
+  // ---- keys -> s_keys; the payload window is written in sorted order at the end: bring it into L2 meanwhile ---------------
+  const range_window kw = range_window_load(s_keys, keys, s, m, mbar_k);
+  if constexpr (!EMU_BUILD) {
+    if (tid == 0 && a.pairs) {
+      const uintptr_t lo = reinterpret_cast<uintptr_t>(vin) & ~uintptr_t(15);
+      const uintptr_t hi = (reinterpret_cast<uintptr_t>(vin + m) + 15) & ~uintptr_t(15);
+      asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(lo), "r"((uint32_t)(hi - lo)) : "memory");
+    }
+    if (kw.bulk) mbar_wait_phase0(mbar_k);
+  }
+  __syncthreads();
+  const UK* sk = s_keys + kw.base;
+
+  // ---- 1. counting pass: bucket histogram, exclusive scan (overflow check), scatter of the local rows ---------------------
+  for (int r = tid; r < m; r += RANGE_THREADS) atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u);
+  __syncthreads();
+  uint32_t c[1 << (RANGE_BUCKET_BITS - 9)];
+  uint32_t tot = 0;
+  bool big = false;
+#pragma unroll
+  for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
+    c[j] = (j < per && tid <= (int)bmask) ? s_cnt[(j << 9) | tid] : 0u;
+    tot += c[j];
+    big = big || c[j] > (uint32_t)RANGE_BUCKET_CAP;
+  }
+  if (big) s_misc[4] = 1;
+  const uint32_t inc = warp_inclusive_sum(tot);
+  if (lane == 31) s_misc[16 + warp] = inc;
+  __syncthreads();
+  if (s_misc[4]) {  // uniform: read by every thread behind the barrier
+    if (tid == 0) atomicOr(&a.ctl->overflow, 1u);
+    return;
+  }
+  {
+    uint32_t run = inc - tot;
+    for (int w = 0; w < warp; ++w) run += s_misc[16 + w];
+#pragma unroll
+    for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
+      if (j < per && tid <= (int)bmask) s_cnt[(j << 9) | tid] = run;
+      run += c[j];
+    }
+  }
+  __syncthreads();
+  for (int r = tid; r < m; r += RANGE_THREADS) s_perm[atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u)] = (uint16_t)r;
+  __syncthreads();
+
+  // ---- 2. the row at bucket position p goes to bucket start + #{bucket rows with a smaller (key, local row)} --------------
+  // (the counters now hold the bucket ends; consecutive positions share buckets, so a warp's walks are mostly broadcasts)
+  uint32_t pk[RANGE_IPT];  // destination | local row << 16
+#pragma unroll
+  for (int i = 0; i < RANGE_IPT; ++i) {
+    const int p = tid + RANGE_THREADS * i;
+    if (p >= m) break;
+    const uint32_t r = s_perm[p];
+    const UK k = sk[r];
+    const uint32_t b = bucket(k);
+    const uint32_t end = s_cnt[slot(b)];
+    const uint32_t start = b ? s_cnt[slot(b - 1)] : 0u;
+    uint32_t before = 0;
+    for (uint32_t q = start; q < end; ++q) {
+      const uint32_t rq = s_perm[q];
+      const UK kq = sk[rq];
+      before += (kq < k || (kq == k && rq < r)) ? 1u : 0u;
+    }
+    pk[i] = (start + before) | r << 16;
+  }
+  __syncthreads();  // the keys (pairs) and the bucket order in s_perm are dead
+
+  // ---- 3. sorted local rows -> s_perm; rows written in order from shared memory ----------------------------------------------
+  range_window vw{0, false};
+  if (a.pairs) vw = range_window_load(s_vals, vin, s, m, mbar_v);
+#pragma unroll
+  for (int i = 0; i < RANGE_IPT; ++i) {
+    if (tid + RANGE_THREADS * i >= m) break;
+    s_perm[pk[i] & 0xffffu] = (uint16_t)(pk[i] >> 16);
+  }
+  if constexpr (!EMU_BUILD) {
+    if (vw.bulk) mbar_wait_phase0(mbar_v);
+  }
+  __syncthreads();
+  if (a.pairs) {
+    const VT* sv = s_vals + vw.base;
+    for (int r = tid; r < m; r += RANGE_THREADS) vout[r] = sv[s_perm[r]];
   } else {
-    for (int q = tid; q < m; q += RANGE_THREADS) s_keys[q] = ld_stream(keys + q);
-  }
-  if constexpr (!EMU_BUILD) {
-    if (bulk) mbar_wait_phase0(mbar);
-  }
-  __syncthreads();
-
-  // ---- stable LSD ranking passes over the range's remaining digits, lowest first; s_perm[pos] = local row --------------
-  // item i of lane l in warp w is position w * 32 * nit + 32 * i + l of the previous order; positions >= m are padding with
-  // digit 255, which the stable ranking puts behind every row
-  const int nit = (m + RANGE_THREADS - 1) / RANGE_THREADS;
-  const int wbase = warp * 32 * nit + lane;
-  uint32_t* my_hist = s_whist + warp * RADIX;
-  bool first = true;
-  for (uint32_t digits = a.ctl->range_digits; digits != 0; digits &= digits - 1) {
-    const int sh = 8 * (__ffs(digits) - 1);
-    uint32_t pk[RANGE_IPT];  // local row | digit << 16
-#pragma unroll
-    for (int i = 0; i < RANGE_IPT; ++i) {
-      if (i >= nit) break;
-      const int q = wbase + 32 * i;
-      const uint32_t r = q < m ? (first ? (uint32_t)q : (uint32_t)s_perm[q]) : 0u;
-      const uint32_t dg = q < m ? (uint32_t)(s_keys[base + r] >> sh) & 255u : 255u;
-      pk[i] = r | dg << 16;
-    }
-#pragma unroll
-    for (int j = 0; j < RADIX / 32; ++j) my_hist[j * 32 + lane] = 0;
-    __syncwarp();
-    auto digit_at = [&](int i) -> unsigned { return pk[i] >> 16; };
-    const int distinct = warp_digit_counts<RANGE_IPT>(digit_at, nit, lane, my_hist);
-    __syncthreads();
-    // digit d of warp w starts at (rows of digits < d) + (rows of digit d in warps < w)
-    uint32_t cnt = 0, inc = 0;
-    if (tid < RADIX) {
-#pragma unroll
-      for (int w = 0; w < RANGE_WARPS; ++w) {
-        const uint32_t c = s_whist[w * RADIX + tid];
-        s_whist[w * RADIX + tid] = cnt;
-        cnt += c;
-      }
-      inc = warp_inclusive_sum(cnt);
-      if (lane == 31) s_misc[8 + warp] = inc;
-    }
-    __syncthreads();
-    if (tid < RADIX) {
-      uint32_t start = inc - cnt;
-      for (int w = 0; w < warp; ++w) start += s_misc[8 + w];
-#pragma unroll
-      for (int w = 0; w < RANGE_WARPS; ++w) s_whist[w * RADIX + tid] += start;
-    }
-    __syncthreads();
-    uint32_t pos[RANGE_IPT];
-    warp_rank<RANGE_IPT>(digit_at, nit, distinct, lane, my_hist, s_bm + warp * RADIX, pos);
-#pragma unroll
-    for (int i = 0; i < RANGE_IPT; ++i) {
-      if (i >= nit) break;
-      if (wbase + 32 * i < m) s_perm[pos[i]] = (uint16_t)(pk[i] & 0xffffu);
-    }
-    __syncthreads();
-    first = false;
-  }
-
-  // ---- segment walk over the bits below fix_shift; a range edge is a segment edge ----------------------------------------
-  const int shift = a.ctl->fix_shift;
-  const UK desc = (UK)a.desc_mask;
-  for (int r = tid; r < m; r += RANGE_THREADS) {
-    const int lr = s_perm[r];
-    const UK k = s_keys[base + lr];
-    const int lmax = min(r, FIX_HALO);
-    const int rmax = min(m - 1 - r, FIX_HALO);
-    const seg_walk w = segment_walk<UK, 0>([&](int o) { return s_keys[base + s_perm[r + o]]; }, k, shift, lmax, rmax);
-    int dst = r - w.left + w.before;
-    if (w.cut) {
-      dst = r;
-      if (!w.all_equal) atomicOr(&a.ctl->overflow, 1u);
-    }
-    if (a.pairs) vout[dst] = vin[lr];
-    else kout[dst] = untwiddle_rt<UK>(k, a.kind, desc);
+    const UK desc = (UK)a.desc_mask;
+    for (int r = tid; r < m; r += RANGE_THREADS) kout[r] = untwiddle_rt<UK>(sk[s_perm[r]], a.kind, desc);
   }
 }
 

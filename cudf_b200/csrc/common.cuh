@@ -277,7 +277,7 @@ void range_partition_counts(const b2_column_view& keys, const void* splitters, i
 void range_partition_scatter(const b2_column_view& keys, const b2_column_view* values, const void* splitters, int P, void* const* key_dst,
                              void* const* val_dst, cudaStream_t stream);
 
-// radix_join.cu (experimental, opt-in: B2_JOIN_RADIX_ROWS)
+// radix_join.cu (the free-function join when both sides have >= 2^24 null-free rows; B2_JOIN_RADIX_ROWS moves the limit)
 bool radix_join_applicable(const std::vector<b2_column_view>& a, const std::vector<b2_column_view>& b);
 void radix_join(const std::vector<b2_column_view>& build, const std::vector<b2_column_view>& probe, bool left, cudaStream_t stream,
                 column_ptr& out_probe, column_ptr& out_build);

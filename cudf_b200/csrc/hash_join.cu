@@ -778,7 +778,7 @@ static b2_status free_join(const b2_table_view* left, const b2_table_view* right
   const bool nulls = table_has_nulls(l) || table_has_nulls(r);
   column_ptr lo, ro;
   // inner join builds on the smaller table and swaps the outputs back (join.cu:52-59)
-  if (radix_join_applicable(l, r)) {  // opt-in partitioned path (radix_join.cu), off by default
+  if (radix_join_applicable(l, r)) {  // partitioned path (radix_join.cu): both sides >= 2^24 null-free rows, keys <= 8 bytes
     make_key_cols(l, true);  // same argument checks as the hash path
     if (kind == JOIN_INNER) {
       if (r[0].size > l[0].size) radix_join(l, r, false, S(stream), ro, lo);

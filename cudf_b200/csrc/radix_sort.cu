@@ -1669,7 +1669,7 @@ void radix_partition_top16(const uint64_t* keys_in, int64_t n, uint64_t* keys_ou
 }
 
 // Same, but `packed_keys` are the raw packed join keys: the kernels apply mix64 on load (histogram of the two
-// needed digits only), so keys_out receives mix64(key) grouped by its top 16 bits. EXPERIMENTAL (radix_join.cu).
+// needed digits only), so keys_out receives mix64(key) grouped by its top 16 bits. Used by the partitioned join (radix_join.cu).
 void radix_partition_top16_mix(const uint64_t* packed_keys, int64_t n, uint64_t* keys_out, int32_t* idx_out, cudaStream_t stream)
 {
   dbuf b(sizeof(uint64_t) * n, stream), it(sizeof(int32_t) * n, stream);

@@ -64,6 +64,57 @@ def test_join_multi_key(cu):
             assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1])
 
 
+def test_wide_keys_join_and_groupby(plc):
+    """Keys wider than 8 bytes: the table holds a hash of the row and confirms it against the key columns."""
+    cu, o = PlcImpl(plc), OracleImpl()
+    rng = np.random.default_rng(91)
+    # join: (int64, int64 with nulls) and (int32, float64 with NaN / -0, int64)
+    for nl, nr in [(1, 1), (20_000, 7_000), (3_000, 50_000)]:
+        l = [(rng.integers(0, 40, nl).astype(np.int64), None), (rng.integers(0, 30, nl).astype(np.int64), rng.random(nl) < 0.9)]
+        r = [(rng.integers(0, 40, nr).astype(np.int64), None), (rng.integers(0, 30, nr).astype(np.int64), rng.random(nr) < 0.9)]
+        for kind in ("inner_join", "left_join", "full_join"):
+            for ne in (0, 1):
+                got, exp = getattr(cu, kind)(l, r, ne), getattr(o, kind)(l, r, ne)
+                assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (nl, nr, kind, ne)
+        assert cu.inner_join_size(l, r) == o.inner_join_size(l, r)
+    # sliced views of both sides (offsets not a multiple of 32): row ids count from the start of the view
+    (lb, le), (rb, re) = (5, 2_990), (37, 49_000)
+    lt = plc.Table([plc.Column.from_numpy(v, m).slice(lb, le) for v, m in l])
+    rt = plc.Table([plc.Column.from_numpy(v, m).slice(rb, re) for v, m in r])
+    ls = [(v[lb:le], None if m is None else m[lb:le]) for v, m in l]
+    rs = [(v[rb:re], None if m is None else m[rb:re]) for v, m in r]
+    for kind in ("inner_join", "left_join", "full_join"):
+        for ne in (0, 1):
+            res = getattr(plc.join, kind)(lt, rt, ne)
+            got = ojoin.canonical(res[0].to_numpy()[0], res[1].to_numpy()[0])
+            exp = getattr(o, kind)(ls, rs, ne)
+            assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), ("sliced", kind, ne)
+    f = np.array([0.0, -0.0, np.nan, 1.5, np.nan, 2.0])
+    l = [(np.arange(6, dtype=np.int32) % 2, None), (f, None), (np.arange(6, dtype=np.int64) % 2, None)]
+    r = [(np.array([0, 1, 0, 1], np.int32), None), (np.array([-0.0, np.nan, np.nan, 1.5]), None), (np.array([0, 1, 0, 1], np.int64), None)]
+    got, exp = cu.inner_join(l, r), o.inner_join(l, r)
+    assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1])
+    # groupby aggregate + scan on (int64, int64) keys
+    n = 60_000
+    keys = [(rng.integers(0, 50, n).astype(np.int64), None), (rng.integers(-20, 20, n).astype(np.int64), rng.random(n) < 0.95)]
+    vals = (rng.integers(-1000, 1000, n).astype(np.int32), rng.random(n) < 0.8)
+    kinds = ["sum", "min", "max", "count", "count_all"]
+    for inc in (False, True):
+        gk, gr = sort_groups(*cu.groupby(keys, [(vals, kinds)], include_nulls=inc))
+        ek, er = sort_groups(*o.groupby(keys, [(vals, kinds)], include_nulls=inc))
+        for a, b in zip(gk, ek):
+            assert_columns_equal(a, b, what="keys")
+        for j, kind in enumerate(kinds):
+            assert_columns_equal(gr[0][j], er[0][j], what=kind)
+    nn = [(keys[0][0], None), (keys[1][0], None)]
+    gk, gr = cu.groupby_scan(nn, [(vals, ["sum", "count"])])
+    ek, er = o.groupby_scan(nn, [(vals, ["sum", "count"])])
+    for a, b in zip(gk, ek):
+        assert_columns_equal(a, b, what="scan keys")
+    for j in range(2):
+        assert_columns_equal(gr[0][j], er[0][j], what=f"scan {j}")
+
+
 def test_hash_join_object_reuse_and_errors(plc):
     rng = np.random.default_rng(44)
     build = (rng.integers(0, 1000, 50_000).astype(np.int64), None)

@@ -170,6 +170,21 @@ def test_sort_by_key_payload(plc):
     assert got.columns()[0].null_count() == int((~vals[0][1]).sum())
 
 
+def test_sort_by_key_carry_payload(plc):
+    """One non-null payload column carried through the passes (no row ids, no gather) for key / value type pairs at the
+    6144-row tile edge."""
+    rng = np.random.default_rng(5)
+    for n in (1, 33, 6144, 6145, 200_003):
+        for kdt in (np.int64, np.int32, np.uint16, np.float64):
+            for vdt in (np.int64, np.float64, np.int32, np.float32):
+                keys = (rng.standard_normal(n) * 50).astype(kdt)
+                vals = rng.integers(0, 1 << 30, n).astype(vdt)
+                for order in ((0, 1) if np.dtype(kdt).kind != "f" else (0,)):
+                    got = plc.sorting.sort_by_key(plc.Table([plc.Column.from_numpy(vals)]), plc.Table([plc.Column.from_numpy(keys)]), [order], [])
+                    exp = osort.sort_by_key([(vals, None)], [(keys, None)], [order])[0][0]
+                    assert np.array_equal(got.columns()[0].to_numpy()[0], exp), (n, kdt, vdt, order)
+
+
 def test_sortedness_property_large(plc):
     """Size-independent properties at 2^26 rows: permutation, non-decreasing keys, stable ties."""
     import torch

@@ -1,6 +1,7 @@
-"""Opt-in experimental paths that were written after the round-1 GPU budget was spent. They are OFF by default; these
-checks run them in a subprocess with their environment switch and are marked xfail(strict=False) so that the first
-hardware run reports their state (XPASS / XFAIL) without gating the validated suite."""
+"""The aliased sort_by_key(T, T) shortcut (B2_SORT_ALIAS=1): the keys are sorted by the keys-only radix sort and the sorted
+keys are the payload. It is opt-in and has not yet been run on hardware, so this check runs it in a subprocess with its switch,
+is skipped unless B2_RUN_EXPERIMENTAL=1, and is marked xfail(strict=False) so that a hardware run reports its state
+(XPASS / XFAIL) without gating the suite."""
 import os
 import subprocess
 import sys
@@ -8,34 +9,10 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-# Never-run code can hang a kernel; the default GPU suite must not depend on it. Set B2_RUN_EXPERIMENTAL=1 to run these.
+# Never-run code can hang a kernel; the default GPU suite must not depend on it. Set B2_RUN_EXPERIMENTAL=1 to run it.
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(os.environ.get("B2_RUN_EXPERIMENTAL", "0") != "1",
-                                 reason="opt-in paths not yet validated on hardware: set B2_RUN_EXPERIMENTAL=1")]
-
-
-@pytest.mark.xfail(strict=False, reason="payload-carrying sort_by_key (B2_SORT_CARRY=1) not yet validated on hardware")
-def test_sort_by_key_carry_payload():
-    code = r"""
-import numpy as np, sys
-sys.path.insert(0, '.')
-import cudf_b200.pylibcudf as plc
-from oracle import sort as osort
-rng = np.random.default_rng(5)
-for n in (1, 33, 6144, 6145, 200_003):
-    for kdt in (np.int64, np.int32, np.uint16, np.float64):
-        for vdt in (np.int64, np.float64, np.int32, np.float32):
-            keys = (rng.standard_normal(n) * 50).astype(kdt)
-            vals = rng.integers(0, 1 << 30, n).astype(vdt)
-            for order in ((0, 1) if np.dtype(kdt).kind != 'f' else (0,)):
-                got = plc.sorting.sort_by_key(plc.Table([plc.Column.from_numpy(vals)]), plc.Table([plc.Column.from_numpy(keys)]), [order], [])
-                exp = osort.sort_by_key([(vals, None)], [(keys, None)], [order])[0][0]
-                assert np.array_equal(got.columns()[0].to_numpy()[0], exp), (n, kdt, vdt, order)
-print('CARRY_OK')
-"""
-    env = dict(os.environ, B2_SORT_CARRY="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
-    assert "CARRY_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-2500:]
+                                 reason="opt-in path not yet validated on hardware: set B2_RUN_EXPERIMENTAL=1")]
 
 
 @pytest.mark.xfail(strict=False, reason="aliased sort_by_key(T, T) -> keys-only radix (B2_SORT_ALIAS=1) not yet run on hardware")
@@ -60,92 +37,3 @@ print('ALIAS_OK')
     env = dict(os.environ, B2_SORT_ALIAS="1")
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
     assert "ALIAS_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-2500:]
-
-
-@pytest.mark.xfail(strict=False, reason="partitioned shared-memory inner join (B2_JOIN_RADIX_ROWS) not yet run on hardware")
-def test_radix_inner_join():
-    code = r"""
-import numpy as np, sys
-sys.path.insert(0, '.')
-import cudf_b200.pylibcudf as plc
-from oracle import join as ojoin
-from tests.impls import PlcImpl
-cu = PlcImpl(plc)
-rng = np.random.default_rng(78)
-def check(l, r, tag):
-    for kind in ("inner_join", "left_join", "full_join"):
-        got = getattr(cu, kind)(l, r); exp = getattr(ojoin, kind)(l, r)
-        assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (tag, kind)
-for dtype in (np.int64, np.int32, np.float64, np.int8):
-    for nl, nr in [(1, 1), (1000, 700), (50_000, 20_000), (300, 90_000), (200_000, 150_000)]:
-        if dtype == np.int8 and nl > 50_000:
-            continue
-        hi = 100 if dtype == np.int8 else 5000 * max(1, nl // 20_000)
-        check([(rng.integers(0, hi, nl).astype(dtype), None)], [(rng.integers(0, hi, nr).astype(dtype), None)], (dtype, nl, nr))
-# wide random keys: almost no matches except planted ones
-l = rng.integers(-2**62, 2**62, 300_000); r = rng.integers(-2**62, 2**62, 250_000); l[::7] = r[rng.integers(0, r.size, l[::7].size)]
-check([(l, None)], [(r, None)], 'wide')
-# one key repeated 40000 times on the build side: its partition is joined in three shared-memory chunks
-b = rng.integers(0, 1000, 60_000); b[:40_000] = 424242
-p = rng.integers(0, 1000, 80_000); p[:30] = 424242
-check([(p, None)], [(b, None)], 'chunks'); check([(b, None)], [(p, None)], 'chunks-swapped')
-# probe-side hot key: its partition is split into several (partition, probe piece) work items
-p = rng.integers(0, 100_000, 400_000); p[:300_000] = 777
-b = rng.integers(0, 100_000, 30_000); b[:5] = 777
-check([(p, None)], [(b, None)], 'probe pieces')
-# two-column packed key
-l = [(rng.integers(0, 50, 20000).astype(np.int32), None), (rng.integers(0, 9, 20000).astype(np.int16), None)]
-r = [(rng.integers(0, 50, 9000).astype(np.int32), None), (rng.integers(0, 9, 9000).astype(np.int16), None)]
-check(l, r, 'two columns')
-# -0.0 == +0.0 and NaN == NaN (row equality of the reference)
-f = np.array([0.0, -0.0, np.nan, 1.5, np.nan]); g = np.array([-0.0, np.nan, 2.5, 0.0])
-check([(f, None)], [(g, None)], 'float specials')
-print('RADIX_JOIN_OK')
-"""
-    env = dict(os.environ, B2_JOIN_RADIX_ROWS="1")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=ROOT, timeout=300)
-    assert "RADIX_JOIN_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-2500:]
-
-
-@pytest.mark.xfail(strict=False, reason="keys wider than 8 bytes (hash + column comparison) not yet run on hardware")
-def test_wide_keys_join_and_groupby(plc):
-    import numpy as np
-
-    from tests.helpers import assert_columns_equal
-    from tests.impls import OracleImpl, PlcImpl, sort_groups
-
-    cu, o = PlcImpl(plc), OracleImpl()
-    rng = np.random.default_rng(91)
-    # join: (int64, int64 with nulls) and (int32, float64 with NaN / -0, int64)
-    for nl, nr in [(1, 1), (20_000, 7_000), (3_000, 50_000)]:
-        l = [(rng.integers(0, 40, nl).astype(np.int64), None), (rng.integers(0, 30, nl).astype(np.int64), rng.random(nl) < 0.9)]
-        r = [(rng.integers(0, 40, nr).astype(np.int64), None), (rng.integers(0, 30, nr).astype(np.int64), rng.random(nr) < 0.9)]
-        for kind in ("inner_join", "left_join", "full_join"):
-            for ne in (0, 1):
-                got, exp = getattr(cu, kind)(l, r, ne), getattr(o, kind)(l, r, ne)
-                assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (nl, nr, kind, ne)
-        assert cu.inner_join_size(l, r) == o.inner_join_size(l, r)
-    f = np.array([0.0, -0.0, np.nan, 1.5, np.nan, 2.0])
-    l = [(np.arange(6, dtype=np.int32) % 2, None), (f, None), (np.arange(6, dtype=np.int64) % 2, None)]
-    r = [(np.array([0, 1, 0, 1], np.int32), None), (np.array([-0.0, np.nan, np.nan, 1.5]), None), (np.array([0, 1, 0, 1], np.int64), None)]
-    got, exp = cu.inner_join(l, r), o.inner_join(l, r)
-    assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1])
-    # groupby aggregate + scan on (int64, int64) keys
-    n = 60_000
-    keys = [(rng.integers(0, 50, n).astype(np.int64), None), (rng.integers(-20, 20, n).astype(np.int64), rng.random(n) < 0.95)]
-    vals = (rng.integers(-1000, 1000, n).astype(np.int32), rng.random(n) < 0.8)
-    kinds = ["sum", "min", "max", "count", "count_all"]
-    for inc in (False, True):
-        gk, gr = sort_groups(*cu.groupby(keys, [(vals, kinds)], include_nulls=inc))
-        ek, er = sort_groups(*o.groupby(keys, [(vals, kinds)], include_nulls=inc))
-        for a, b in zip(gk, ek):
-            assert_columns_equal(a, b, what="keys")
-        for j, kind in enumerate(kinds):
-            assert_columns_equal(gr[0][j], er[0][j], what=kind)
-    nn = [(keys[0][0], None), (keys[1][0], None)]
-    gk, gr = cu.groupby_scan(nn, [(vals, ["sum", "count"])])
-    ek, er = o.groupby_scan(nn, [(vals, ["sum", "count"])])
-    for a, b in zip(gk, ek):
-        assert_columns_equal(a, b, what="scan keys")
-    for j in range(2):
-        assert_columns_equal(gr[0][j], er[0][j], what=f"scan {j}")

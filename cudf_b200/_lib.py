@@ -136,6 +136,10 @@ _sig("b2_hash_join_partitioned_join", [vp, P(TableView), P(ColumnView), i32, i32
 _sig("b2_hash_join_finalize_full_join", [P(ColumnView), P(ColumnView), i32, i32, i32, b2_stream, P(vp), P(vp)])
 _sig("b2_hash_join_create", [P(TableView), i32, i32, C.c_double, b2_stream, P(vp)])
 _sig("b2_hash_join_destroy", [vp], None)
+_sig("b2_filtered_join_create", [P(TableView), i32, C.c_double, b2_stream, P(vp)])
+_sig("b2_filtered_join_destroy", [vp], None)
+_sig("b2_filtered_join_semi_join", [vp, P(TableView), b2_stream, P(vp)])
+_sig("b2_filtered_join_anti_join", [vp, P(TableView), b2_stream, P(vp)])
 _sig("b2_groupby_create", [P(TableView), i32, i32, u8p, i32, u8p, i32, P(vp)])
 _sig("b2_groupby_destroy", [vp], None)
 _sig("b2_groupby_aggregate", [vp, P(AggRequest), i32, b2_stream, P(vp), P(vp)])
@@ -188,7 +192,8 @@ DECLARED_SYMBOLS = [
     "b2_ipc_free", "b2_peer_copy", "b2_profile_get_over", "b2_hash_partition", "b2_partition_by_map", "b2_range_partition_counts", "b2_range_partition_scatter", "b2_packed_size", "b2_pack", "b2_pack_metadata", "b2_unpack", "b2_to_arrow_schema", "b2_to_arrow_device", "b2_to_arrow_host", "b2_from_arrow_device",
     "b2_from_arrow_host", "b2_arrow_schema_release", "b2_arrow_array_release",
     "b2_fill_splitmix64", "b2_apply_boolean_mask", "b2_drop_nulls", "b2_drop_nans", "b2_unique", "b2_distinct",
-    "b2_distinct_indices",
+    "b2_distinct_indices", "b2_filtered_join_create", "b2_filtered_join_destroy", "b2_filtered_join_semi_join",
+    "b2_filtered_join_anti_join",
 ]
 
 

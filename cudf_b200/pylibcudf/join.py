@@ -1,4 +1,4 @@
-"""pylibcudf.join twin (python/pylibcudf/pylibcudf/join.pyx:63-205) + cudf::hash_join object."""
+"""pylibcudf.join twin (python/pylibcudf/pylibcudf/join.pyx:63-306) + the cudf::hash_join and cudf::filtered_join objects."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,6 +26,46 @@ def left_join(left_keys: Table, right_keys: Table, nulls_equal: NullEquality, st
 
 def full_join(left_keys: Table, right_keys: Table, nulls_equal: NullEquality, stream=None, mr=None):
     return _free_join("b2_full_join", left_keys, right_keys, nulls_equal, stream)
+
+
+def left_semi_join(left_keys: Table, right_keys: Table, nulls_equal: NullEquality, stream=None, mr=None) -> Column:
+    """INT32 indices of the left rows equal to some right row, ascending (join.pyx:207-256: a FilteredJoin probed once)."""
+    return FilteredJoin(right_keys, nulls_equal, stream=stream).semi_join(left_keys, stream)
+
+
+def left_anti_join(left_keys: Table, right_keys: Table, nulls_equal: NullEquality, stream=None, mr=None) -> Column:
+    """INT32 indices of the left rows equal to no right row, ascending (join.pyx:259-306)."""
+    return FilteredJoin(right_keys, nulls_equal, stream=stream).anti_join(left_keys, stream)
+
+
+class FilteredJoin:
+    """cudf::filtered_join (cpp/include/cudf/join/filtered_join.hpp): the right (filter) table's keys become a distinct set
+    once; semi_join / anti_join probe it with any number of left tables. Keeps `right` alive: keys wider than 8 bytes are
+    compared against its columns."""
+
+    def __init__(self, right: Table, compare_nulls: NullEquality, load_factor: float = 0.5, stream=None):
+        self._right = right
+        out = C.c_void_p()
+        rv = right._view()
+        check(lib.b2_filtered_join_create(C.byref(rv), int(compare_nulls), float(load_factor), _lib.stream_arg(stream), C.byref(out)))
+        self._handle = out.value
+
+    def _probe(self, name, left, stream):
+        out = C.c_void_p()
+        lv = left._view()
+        check(getattr(lib, name)(C.c_void_p(self._handle), C.byref(lv), _lib.stream_arg(stream), C.byref(out)))
+        return Column._from_handle(out.value)
+
+    def semi_join(self, left: Table, stream=None, mr=None) -> Column:
+        return self._probe("b2_filtered_join_semi_join", left, stream)
+
+    def anti_join(self, left: Table, stream=None, mr=None) -> Column:
+        return self._probe("b2_filtered_join_anti_join", left, stream)
+
+    def __del__(self):
+        if getattr(self, "_handle", 0):
+            lib.b2_filtered_join_destroy(C.c_void_p(self._handle))
+            self._handle = 0
 
 
 class HashJoin:

@@ -613,6 +613,60 @@ cdef class HashJoin:
         return finalize_partitioned_full_join(left_partials, right_partials, left_table_num_rows, right_table_num_rows, stream)
 
 
+ctypedef b2_status (*filtered_probe_fn)(const b2_filtered_join*, const b2_table_view*, b2_stream, b2_column**) noexcept nogil
+
+
+cdef class FilteredJoin:
+    """cudf::filtered_join (cpp/include/cudf/join/filtered_join.hpp): the right (filter) table's keys become a distinct set
+    once; semi_join / anti_join return the ascending INT32 indices of the left rows with / without an equal right row."""
+    cdef b2_filtered_join* fj
+    cdef object right
+
+    def __cinit__(self):
+        self.fj = NULL
+
+    def __init__(self, Table right, compare_nulls, double load_factor=0.5, stream=None):
+        cdef _TableView rv = _TableView.of(right)
+        cdef int32_t cn = int(compare_nulls)
+        cdef b2_stream s = _stream(stream)
+        cdef b2_status st
+        self.right = right  # keys wider than 8 bytes are compared against its columns
+        with nogil:
+            st = b2_filtered_join_create(&rv.tv, cn, load_factor, s, &self.fj)
+        check(st)
+
+    def __dealloc__(self):
+        if self.fj != NULL:
+            b2_filtered_join_destroy(self.fj)
+            self.fj = NULL
+
+    cdef Column _probe(self, filtered_probe_fn fn, Table left, object stream):
+        cdef _TableView lv = _TableView.of(left)
+        cdef b2_stream s = _stream(stream)
+        cdef b2_column* out = NULL
+        cdef b2_status st
+        with nogil:
+            st = fn(self.fj, &lv.tv, s, &out)
+        check(st)
+        return Column.from_handle(out)
+
+    def semi_join(self, Table left, stream=None, mr=None):
+        return self._probe(b2_filtered_join_semi_join, left, stream)
+
+    def anti_join(self, Table left, stream=None, mr=None):
+        return self._probe(b2_filtered_join_anti_join, left, stream)
+
+
+def left_semi_join(Table left_keys, Table right_keys, nulls_equal, stream=None, mr=None):
+    """join.pyx:207-256: a FilteredJoin of `right_keys` probed once."""
+    return FilteredJoin(right_keys, nulls_equal, stream=stream).semi_join(left_keys, stream)
+
+
+def left_anti_join(Table left_keys, Table right_keys, nulls_equal, stream=None, mr=None):
+    """join.pyx:259-306: a FilteredJoin of `right_keys` probed once."""
+    return FilteredJoin(right_keys, nulls_equal, stream=stream).anti_join(left_keys, stream)
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # groupby (python/pylibcudf/pylibcudf/groupby.pyx:36-243)
 # ---------------------------------------------------------------------------------------------------------------------

@@ -27,6 +27,7 @@ cdef extern from "cudf_b200.h" nogil:
     ctypedef struct b2_scalar
     ctypedef struct b2_groupby
     ctypedef struct b2_hash_join
+    ctypedef struct b2_filtered_join
 
     ctypedef struct b2_agg_request:
         b2_column_view values
@@ -81,6 +82,13 @@ cdef extern from "cudf_b200.h" nogil:
     b2_status b2_hash_join_inner_join_size(const b2_hash_join* hj, const b2_table_view* probe, b2_stream stream, size_t* out)
     b2_status b2_hash_join_left_join_size(const b2_hash_join* hj, const b2_table_view* probe, b2_stream stream, size_t* out)
     b2_status b2_hash_join_full_join_size(const b2_hash_join* hj, const b2_table_view* probe, b2_stream stream, size_t* out)
+
+    # semi / anti joins (cpp/include/cudf/join/filtered_join.hpp)
+    b2_status b2_filtered_join_create(const b2_table_view* right, int32_t compare_nulls, double load_factor, b2_stream stream,
+                                      b2_filtered_join** out)
+    void b2_filtered_join_destroy(b2_filtered_join* fj)
+    b2_status b2_filtered_join_semi_join(const b2_filtered_join* fj, const b2_table_view* left, b2_stream stream, b2_column** out)
+    b2_status b2_filtered_join_anti_join(const b2_filtered_join* fj, const b2_table_view* left, b2_stream stream, b2_column** out)
 
     # groupby (cpp/include/cudf/groupby.hpp:54-184)
     b2_status b2_groupby_create(const b2_table_view* keys, int32_t null_handling, int32_t keys_are_sorted, const uint8_t* column_order,

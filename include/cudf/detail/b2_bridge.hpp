@@ -595,6 +595,48 @@ class hash_join {
   b2_hash_join* h_{nullptr};
 };
 
+// join/filtered_join.hpp: left semi / anti join against a right (filter) table built once; results are the left row
+// indices in ascending order. load_factor outside (0, 1] is std::invalid_argument.
+class filtered_join {
+ public:
+  filtered_join() = delete;
+  filtered_join(filtered_join const&)            = delete;
+  filtered_join(filtered_join&&)                 = delete;
+  filtered_join& operator=(filtered_join const&) = delete;
+  filtered_join& operator=(filtered_join&&)      = delete;
+  filtered_join(table_view const& right, null_equality compare_nulls, rmm::cuda_stream_view stream)
+    : filtered_join(right, compare_nulls, 0.5, stream)
+  {
+  }
+  filtered_join(table_view const& right, null_equality compare_nulls, double load_factor, rmm::cuda_stream_view stream)
+  {
+    auto r = right.native();
+    detail::check(b2_filtered_join_create(&r, static_cast<int32_t>(compare_nulls), load_factor, stream.value(), &h_));
+  }
+  ~filtered_join() { if (h_) b2_filtered_join_destroy(h_); }
+  [[nodiscard]] std::unique_ptr<rmm::device_uvector<size_type>> semi_join(
+    table_view const& left, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+    rmm::device_async_resource_ref = cudf::get_current_device_resource_ref()) const
+  {
+    auto l = left.native();
+    b2_column* out = nullptr;
+    detail::check(b2_filtered_join_semi_join(h_, &l, stream.value(), &out));
+    return detail::to_uvector(out);
+  }
+  [[nodiscard]] std::unique_ptr<rmm::device_uvector<size_type>> anti_join(
+    table_view const& left, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+    rmm::device_async_resource_ref = cudf::get_current_device_resource_ref()) const
+  {
+    auto l = left.native();
+    b2_column* out = nullptr;
+    detail::check(b2_filtered_join_anti_join(h_, &l, stream.value(), &out));
+    return detail::to_uvector(out);
+  }
+
+ private:
+  b2_filtered_join* h_{nullptr};
+};
+
 // ------------------------------------------------------------------------------------------------
 // groupby.hpp
 // ------------------------------------------------------------------------------------------------

@@ -99,6 +99,7 @@ typedef struct b2_table     b2_table;     /* owning cudf::table      (table.hpp:
 typedef struct b2_scalar    b2_scalar;    /* owning numeric_scalar<T> (scalar/scalar.hpp) */
 typedef struct b2_buffer    b2_buffer;    /* owning rmm::device_buffer                    */
 typedef struct b2_hash_join b2_hash_join; /* cudf::hash_join         (join/hash_join.hpp) */
+typedef struct b2_filtered_join b2_filtered_join;   /* cudf::filtered_join (join/filtered_join.hpp) */
 typedef struct b2_groupby   b2_groupby;   /* cudf::groupby::groupby  (groupby.hpp)        */
 
 /* cudf::groupby::aggregation_request (cpp/include/cudf/groupby.hpp:60-64) */
@@ -257,6 +258,25 @@ B2_API b2_status b2_hash_join_finalize_full_join(const b2_column_view* left_part
                                                  const b2_column_view* right_partials, int32_t num_partials,
                                                  int32_t left_table_num_rows, int32_t right_table_num_rows,
                                                  b2_stream stream, b2_column** out_left, b2_column** out_right);
+
+/* ---- semi / anti join: cpp/include/cudf/join/filtered_join.hpp, cpp/src/join/filtered_join/filtered_join.cu ---------------
+ * The right (filter) table's key rows form a distinct set built once; semi_join returns the INT32 indices of the left rows
+ * equal to some right row, anti_join those equal to none, both strictly ascending.  Row equality is the hash join's (NaN ==
+ * NaN, -0 == +0); compare_nulls = null_equality (0 EQUAL: null == null; 1 UNEQUAL: a row with a null key matches nothing,
+ * so it is in the anti result).  semi_join of an empty side is empty; anti_join of an empty left side is empty and against
+ * an empty right side is 0..n-1.  load_factor outside (0, 1] -> INVALID_ARGUMENT (the reference's default is 0.5); the set
+ * has the smallest power of two >= max(rows + 1, rows / load_factor) slots of 16 bytes, at most 8x the smallest power of
+ * two above the row count and at most 2^31.  Key column count or type differing from the right table's ->
+ * INVALID_ARGUMENT; more than 8 key columns -> INVALID_ARGUMENT; a non-fixed-width column -> DATA_TYPE.  The object is
+ * immutable: probes may run concurrently from several threads / streams once construction has completed on its stream.
+ * With keys wider than 8 bytes the right table's memory must outlive the object. */
+B2_API b2_status b2_filtered_join_create(const b2_table_view* right, int32_t compare_nulls, double load_factor,
+                                         b2_stream stream, b2_filtered_join** out);
+B2_API void      b2_filtered_join_destroy(b2_filtered_join* fj);
+B2_API b2_status b2_filtered_join_semi_join(const b2_filtered_join* fj, const b2_table_view* left, b2_stream stream,
+                                            b2_column** out);
+B2_API b2_status b2_filtered_join_anti_join(const b2_filtered_join* fj, const b2_table_view* left, b2_stream stream,
+                                            b2_column** out);
 
 /* ---- groupby: cpp/include/cudf/groupby.hpp:121-125,181-184, cpp/src/groupby/groupby.cu ----- */
 B2_API b2_status b2_groupby_create(const b2_table_view* keys, int32_t null_handling, int32_t keys_are_sorted,

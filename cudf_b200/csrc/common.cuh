@@ -263,7 +263,6 @@ column_ptr sort_single_column(const b2_column_view& col, bool ascending, cudaStr
 bool is_radix_sortable(const b2_column_view& c);
 bool sort_carry_applicable(const b2_column_view& keys, const b2_column_view& values, bool ascending);
 column_ptr sort_by_key_carry(const b2_column_view& keys, const b2_column_view& values, bool ascending, cudaStream_t stream);
-void radix_partition_top16(const uint64_t* keys_in, int64_t n, uint64_t* keys_out, int32_t* idx_out, cudaStream_t stream);
 void radix_partition_top16_mix(const uint64_t* packed_keys, int64_t n, uint64_t* keys_out, int32_t* idx_out, cudaStream_t stream);
 
 void radix_partition_mix_carry(const uint64_t* keys, const void* vals, int val_bytes, int64_t n, uint64_t* mixed_keys_out, void* vals_out,

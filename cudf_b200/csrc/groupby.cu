@@ -822,12 +822,7 @@ void groupby_aggregate(const b2_groupby& gb, const std::vector<request_view>& re
       pa.n = (uint32_t)n;
       pa.item_start = pgb_items.as<uint32_t>();
       pa.item_counter = pgb_items.as<uint32_t>() + 257;
-      static const uint32_t chunk_rows = [] {  // tuning knob: rows per work item (each item merges its groups into the global table once)
-        const char* e = std::getenv("B2_GROUPBY_CHUNK");
-        const long long v = e ? std::atoll(e) : 0;
-        return (v >= 1024 && v <= (1ll << 24)) ? (uint32_t)v : 0u;
-      }();
-      pa.chunk = chunk_rows ? chunk_rows : pgb_chunk_rows(n);
+      pa.chunk = pgb_chunk_rows(n);
       pa.nops = ops.n;
       for (int k = 0; k < ops.n; ++k) {
         pa.op[k] = ops.op[k].op; pa.acc[k] = ops.op[k].acc; pa.accum[k] = ops.op[k].accum; pa.init[k] = acc_init(ops.op[k].acc, ops.op[k].op);

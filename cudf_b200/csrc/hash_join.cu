@@ -22,67 +22,24 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdlib>
 
 namespace b2 {
 namespace {
 
-// Where a kernel takes its keys from.  Classic table: keys are packed on the fly from the key columns and the
-// slot is the low bits of a hash.  "Mixed" table (large builds without null keys): the table stores
-// h = mix64(packed key) — a bijection, so h equality is key equality — and the slot is the TOP bits of h;
-// build / probe rows may arrive pre-mixed and radix-partitioned by the top 16 bits of h
-// (radix_partition_top16) so that consecutive rows touch one ~512 KB region of the table (L2 hits instead of a
-// 128-byte HBM fetch per row).
-struct key_src {
-  key_cols kc;             // used when hkeys == nullptr
-  const uint64_t* hkeys;   // pre-mixed keys (partition order) or null
-  const int32_t* rowids;   // original row of hkeys[r] (null: r)
-  int32_t mixed_shift;     // 0: classic table; else slot = h >> mixed_shift
-};
-
-__device__ __forceinline__ void fetch_key(const key_src& ks, int64_t r, uint64_t& key, uint32_t& nb, int32_t& orig)
-{
-  if (ks.hkeys) {
-    key  = ks.hkeys[r];
-    nb   = 0;
-    orig = ks.rowids ? ks.rowids[r] : (int32_t)r;
-  } else {
-    pack_row(ks.kc, r, key, nb);
-    if (ks.mixed_shift) key = mix64(key);
-    orig = (int32_t)r;
-  }
-}
-__device__ __forceinline__ uint32_t first_slot(const key_src& ks, uint64_t key, uint32_t nb, uint32_t mask)
-{
-  return ks.mixed_shift ? ((uint32_t)(key >> ks.mixed_shift) & mask) : slot_hash(key, nb, mask);
-}
-
-__global__ void __launch_bounds__(256) mix_pack_kernel(key_cols kc, int64_t n, uint64_t* __restrict__ hkeys)
-{
-  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += stride) {
-    uint64_t key;
-    uint32_t nb;
-    pack_row(kc, r, key, nb);
-    hkeys[r] = mix64(key);
-  }
-}
-
-__global__ void __launch_bounds__(256) build_kernel(key_src ks, int64_t n, bool skip_nulls, slot_t* __restrict__ table,
+__global__ void __launch_bounds__(256) build_kernel(key_cols kc, int64_t n, bool skip_nulls, slot_t* __restrict__ table,
                                                     uint32_t mask)
 {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += stride) {
     uint64_t key;
     uint32_t nb;
-    int32_t orig;
-    fetch_key(ks, r, key, nb, orig);
+    pack_row(kc, r, key, nb);
     if (skip_nulls && nb) continue;
-    uint32_t i = first_slot(ks, key, nb, mask);
+    uint32_t i = slot_hash(key, nb, mask);
     while (true) {
-      int old = atomicCAS(&table[i].row, -1, orig);
+      int old = atomicCAS(&table[i].row, -1, (int32_t)r);
       if (old == -1) {
-        slot_t s{key, orig, nb};
+        slot_t s{key, (int32_t)r, nb};
         int4 v;
         memcpy(&v, &s, 16);
         *reinterpret_cast<int4*>(&table[i]) = v;
@@ -93,9 +50,9 @@ __global__ void __launch_bounds__(256) build_kernel(key_src ks, int64_t n, bool 
   }
 }
 
-// counts[r] = number of build rows equal to probe row r (r in the order of `ks`); total += output rows
+// counts[r] = number of build rows equal to probe row r; total += output rows
 template <bool LEFT>
-__global__ void __launch_bounds__(256) count_kernel(key_src ks, int64_t n, bool skip_nulls, bool table_has_null_rows,
+__global__ void __launch_bounds__(256) count_kernel(key_cols kc, int64_t n, bool skip_nulls, bool table_has_null_rows,
                                                     const slot_t* __restrict__ table, uint32_t mask, int32_t* __restrict__ counts,
                                                     unsigned long long* __restrict__ total)
 {
@@ -104,11 +61,10 @@ __global__ void __launch_bounds__(256) count_kernel(key_src ks, int64_t n, bool 
   for (int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += stride) {
     uint64_t key;
     uint32_t nb;
-    int32_t orig;
-    fetch_key(ks, r, key, nb, orig);
+    pack_row(kc, r, key, nb);
     uint32_t c = 0;
     if (!(nb && (skip_nulls || !table_has_null_rows)) && table != nullptr) {
-      uint32_t i = first_slot(ks, key, nb, mask);
+      uint32_t i = slot_hash(key, nb, mask);
       while (true) {
         const slot_t s = load_slot(&table[i]);
         if (s.row == -1) break;
@@ -133,7 +89,7 @@ __global__ void left_adjust_kernel(const int32_t* __restrict__ counts, int64_t n
 }
 
 template <bool LEFT>
-__global__ void __launch_bounds__(256) retrieve_kernel(key_src ks, int64_t n, const slot_t* __restrict__ table, uint32_t mask,
+__global__ void __launch_bounds__(256) retrieve_kernel(key_cols kc, int64_t n, const slot_t* __restrict__ table, uint32_t mask,
                                                        const int32_t* __restrict__ counts, const int32_t* __restrict__ offsets,
                                                        int32_t* __restrict__ out_left, int32_t* __restrict__ out_right)
 {
@@ -143,21 +99,20 @@ __global__ void __launch_bounds__(256) retrieve_kernel(key_src ks, int64_t n, co
     if (c == 0 && !LEFT) continue;
     uint64_t key;
     uint32_t nb;
-    int32_t orig;
-    fetch_key(ks, r, key, nb, orig);
+    pack_row(kc, r, key, nb);
     int32_t o = offsets[r];
     if (c == 0) {
-      out_left[o]  = orig;
+      out_left[o]  = (int32_t)r;
       out_right[o] = B2_JOIN_NO_MATCH;
       continue;
     }
     const int32_t end = o + c;
-    uint32_t i = first_slot(ks, key, nb, mask);
+    uint32_t i = slot_hash(key, nb, mask);
     while (o < end) {
       const slot_t s = load_slot(&table[i]);
       if (s.row == -1) break;
       if (s.key == key && s.nullbits == nb) {
-        out_left[o]  = orig;
+        out_left[o]  = (int32_t)r;
         out_right[o] = s.row;
         ++o;
       }
@@ -259,7 +214,7 @@ __global__ void __launch_bounds__(256) retrieve_wide_kernel(key_cols pk, key_col
 // match counts of a join_match_context. For LEFT the counts are >= 1 (an unmatched row owns one output slot), so an
 // unmatched row is recognised by walking its chain without a hit. Offsets are local to the partition.
 template <bool LEFT, bool WIDE>
-__global__ void __launch_bounds__(256) retrieve_part_kernel(key_src ks, key_cols bk, int64_t row_begin, int64_t n,
+__global__ void __launch_bounds__(256) retrieve_part_kernel(key_cols pk, key_cols bk, int64_t row_begin, int64_t n,
                                                             const slot_t* __restrict__ table, uint32_t mask,
                                                             const int32_t* __restrict__ counts, const int32_t* __restrict__ offsets,
                                                             int32_t* __restrict__ out_left, int32_t* __restrict__ out_right)
@@ -271,21 +226,20 @@ __global__ void __launch_bounds__(256) retrieve_part_kernel(key_src ks, key_cols
     if (c == 0) continue;  // inner context: no match
     uint64_t key;
     uint32_t nb;
-    int32_t orig = (int32_t)r;
-    if constexpr (WIDE) hash_row_wide(ks.kc, r, key, nb);
-    else fetch_key(ks, r, key, nb, orig);
+    if constexpr (WIDE) hash_row_wide(pk, r, key, nb);
+    else pack_row(pk, r, key, nb);
     int32_t o = offsets[i];
     const int32_t end = o + c;
     bool any = false;
     if (table != nullptr) {
-      uint32_t s0 = WIDE ? slot_hash(key, nb, mask) : first_slot(ks, key, nb, mask);
+      uint32_t s0 = slot_hash(key, nb, mask);
       while (o < end) {
         const slot_t s = load_slot(&table[s0]);
         if (s.row == -1) break;
         bool hit = s.key == key && s.nullbits == nb;
-        if constexpr (WIDE) hit = hit && rows_equal_wide(ks.kc, r, bk, s.row);
+        if constexpr (WIDE) hit = hit && rows_equal_wide(pk, r, bk, s.row);
         if (hit) {
-          out_left[o]  = orig;
+          out_left[o]  = (int32_t)r;
           out_right[o] = s.row;
           ++o;
           any = true;
@@ -294,7 +248,7 @@ __global__ void __launch_bounds__(256) retrieve_part_kernel(key_src ks, key_cols
       }
     }
     if (LEFT && !any) {
-      out_left[o]  = orig;
+      out_left[o]  = (int32_t)r;
       out_right[o] = B2_JOIN_NO_MATCH;
     }
   }
@@ -359,7 +313,6 @@ struct b2_hash_join {
   bool has_nulls     = false;  // nullable_join
   int32_t compare_nulls = B2_NULLS_EQUAL;
   uint32_t mask      = 0;
-  int32_t mixed_shift = 0;     // > 0: "mixed" table (keys = mix64(packed key), slot = top bits)
   bool table_has_null_rows = false;
   bool wide = false;           // keys wider than 8 bytes: hash in the slot + column comparison (build_cols must stay alive,
                                // like the reference's build table: hash_join.hpp "must outlive this object")
@@ -370,19 +323,6 @@ struct b2_hash_join {
 namespace b2 {
 
 enum join_kind { JOIN_INNER = 0, JOIN_LEFT = 1, JOIN_FULL = 2 };
-
-// Builds / probes at least this large take the mixed-key, radix-partitioned path. At 1e9 x 1e9 rows the probe count
-// pass gets faster, but the two partition passes per side cost more than that and the build keeps its first-touch
-// atomics on the table lines, so the path is OFF by default (B2_JOIN_PARTITION_ROWS=<rows> enables it; covered by
-// tests/test_parity_gpu.py::test_join_partitioned_path_small).
-static int64_t join_partition_threshold()
-{
-  static int64_t v = [] {
-    const char* e = std::getenv("B2_JOIN_PARTITION_ROWS");
-    return e ? std::atoll(e) : INT64_MAX;
-  }();
-  return v;
-}
 
 static bool table_has_nulls(const std::vector<b2_column_view>& cols)
 {
@@ -417,32 +357,10 @@ b2_hash_join* hash_join_create(const std::vector<b2_column_view>& build, int has
   const bool skip_nulls = compare_nulls == B2_NULLS_UNEQUAL;
   const int64_t n = hj->build_rows;
   hj->table_has_null_rows = table_has_nulls(build) && !skip_nulls;
-  int log2s = 0;
-  while ((1ull << log2s) < slots) ++log2s;
-  // large builds without null keys: mixed table + rows pre-partitioned by the top 16 bits of the mixed key
-  const bool mixed = !hj->wide && !table_has_nulls(build) && n >= join_partition_threshold();
-  key_src ks{};
-  ks.kc = kc;
-  dbuf hk, hk_sorted, ids;
-  if (mixed) {
-    hj->mixed_shift = 64 - log2s;
-    ks.mixed_shift  = hj->mixed_shift;
-    hk        = dbuf(sizeof(uint64_t) * n, stream);
-    hk_sorted = dbuf(sizeof(uint64_t) * n, stream);
-    ids       = dbuf(sizeof(int32_t) * n, stream);
-    {
-      prof_scope ps("join_partition", stream);
-      B2_LAUNCH(mix_pack_kernel, grid_for(n), 256, 0, stream, kc, n, hk.as<uint64_t>());
-      radix_partition_top16(hk.as<uint64_t>(), n, hk_sorted.as<uint64_t>(), ids.as<int32_t>(), stream);
-    }
-    hk.reset();
-    ks.hkeys  = hk_sorted.as<uint64_t>();
-    ks.rowids = ids.as<int32_t>();
-  }
   {
     prof_scope ps("join_build", stream);
     if (hj->wide) B2_LAUNCH(build_wide_kernel, grid_for(n), 256, 0, stream, kc, n, skip_nulls, hj->table.as<slot_t>(), hj->mask);
-    else B2_LAUNCH(build_kernel, grid_for(n), 256, 0, stream, ks, n, skip_nulls, hj->table.as<slot_t>(), hj->mask);
+    else B2_LAUNCH(build_kernel, grid_for(n), 256, 0, stream, kc, n, skip_nulls, hj->table.as<slot_t>(), hj->mask);
   }
   return hj.release();
 }
@@ -463,7 +381,7 @@ struct probe_counts {
   size_t total = 0;
 };
 
-static probe_counts run_count(const b2_hash_join& hj, const key_src& ks, int64_t n, bool left, bool keep_counts,
+static probe_counts run_count(const b2_hash_join& hj, const key_cols& kc, int64_t n, bool left, bool keep_counts,
                               cudaStream_t stream)
 {
   probe_counts pc;
@@ -478,16 +396,16 @@ static probe_counts run_count(const b2_hash_join& hj, const key_src& ks, int64_t
     if (hj.wide) {
       const key_cols bk = make_key_cols(hj.build_cols, true);
       if (left)
-        B2_LAUNCH((count_wide_kernel<true>), grid_for(n), 256, 0, stream, ks.kc, bk, n, skip_nulls, hj.table_has_null_rows, table,
+        B2_LAUNCH((count_wide_kernel<true>), grid_for(n), 256, 0, stream, kc, bk, n, skip_nulls, hj.table_has_null_rows, table,
                   hj.mask, pc.counts.as<int32_t>(), tot.as<unsigned long long>());
       else
-        B2_LAUNCH((count_wide_kernel<false>), grid_for(n), 256, 0, stream, ks.kc, bk, n, skip_nulls, hj.table_has_null_rows, table,
+        B2_LAUNCH((count_wide_kernel<false>), grid_for(n), 256, 0, stream, kc, bk, n, skip_nulls, hj.table_has_null_rows, table,
                   hj.mask, pc.counts.as<int32_t>(), tot.as<unsigned long long>());
     } else if (left)
-      B2_LAUNCH((count_kernel<true>), grid_for(n), 256, 0, stream, ks, n, skip_nulls, hj.table_has_null_rows, table, hj.mask,
+      B2_LAUNCH((count_kernel<true>), grid_for(n), 256, 0, stream, kc, n, skip_nulls, hj.table_has_null_rows, table, hj.mask,
                 pc.counts.as<int32_t>(), tot.as<unsigned long long>());
     else
-      B2_LAUNCH((count_kernel<false>), grid_for(n), 256, 0, stream, ks, n, skip_nulls, hj.table_has_null_rows, table, hj.mask,
+      B2_LAUNCH((count_kernel<false>), grid_for(n), 256, 0, stream, kc, n, skip_nulls, hj.table_has_null_rows, table, hj.mask,
                 pc.counts.as<int32_t>(), tot.as<unsigned long long>());
   }
   unsigned long long h = 0;
@@ -500,35 +418,11 @@ static probe_counts run_count(const b2_hash_join& hj, const key_src& ks, int64_t
 void hash_join_probe(const b2_hash_join* hj, const std::vector<b2_column_view>& probe, int kind, bool has_size, size_t size_hint,
                      cudaStream_t stream, column_ptr& out_left, column_ptr& out_right);
 
-// key source of a probe table: pre-mixed and partitioned when the table is "mixed" and the probe is large
-struct probe_keys {
-  key_src ks{};
-  dbuf hk_sorted, ids;
-};
-static void make_probe_keys(const b2_hash_join& hj, const std::vector<b2_column_view>& probe, cudaStream_t stream, probe_keys& pk)
-{
-  const int64_t n = probe[0].size;
-  pk.ks.kc = make_key_cols(probe, hj.wide);
-  pk.ks.mixed_shift = hj.mixed_shift;
-  if (hj.mixed_shift && !table_has_nulls(probe) && n >= join_partition_threshold()) {
-    dbuf hk(sizeof(uint64_t) * n, stream);
-    pk.hk_sorted = dbuf(sizeof(uint64_t) * n, stream);
-    pk.ids       = dbuf(sizeof(int32_t) * n, stream);
-    prof_scope ps("join_partition", stream);
-    B2_LAUNCH(mix_pack_kernel, grid_for(n), 256, 0, stream, pk.ks.kc, n, hk.as<uint64_t>());
-    radix_partition_top16(hk.as<uint64_t>(), n, pk.hk_sorted.as<uint64_t>(), pk.ids.as<int32_t>(), stream);
-    pk.ks.hkeys  = pk.hk_sorted.as<uint64_t>();
-    pk.ks.rowids = pk.ids.as<int32_t>();
-  }
-}
-
 size_t hash_join_size(const b2_hash_join* hj, const std::vector<b2_column_view>& probe, int kind, cudaStream_t stream)
 {
   validate_probe(*hj, probe);
   const int64_t n = probe[0].size;
-  probe_keys pkeys;
-  make_probe_keys(*hj, probe, stream, pkeys);
-  const key_src& kc = pkeys.ks;
+  const key_cols kc = make_key_cols(probe, hj->wide);
   if (kind == JOIN_INNER) {
     if (n == 0 || hj->build_rows == 0) return 0;
     return run_count(*hj, kc, n, false, false, stream).total;
@@ -547,9 +441,7 @@ void hash_join_probe(const b2_hash_join* hj, const std::vector<b2_column_view>& 
   (void)has_size; (void)size_hint;  // the size is always recomputed: the count pass also yields the offsets
   validate_probe(*hj, probe);
   const int64_t n = probe[0].size;
-  probe_keys pkeys;
-  make_probe_keys(*hj, probe, stream, pkeys);
-  const key_src& kc = pkeys.ks;
+  const key_cols kc = make_key_cols(probe, hj->wide);
   const bool left = kind != JOIN_INNER;
 
   size_t m = 0;
@@ -583,10 +475,10 @@ void hash_join_probe(const b2_hash_join* hj, const std::vector<b2_column_view>& 
     if (hj->wide) {
       const key_cols bk = make_key_cols(hj->build_cols, true);
       if (left)
-        B2_LAUNCH((retrieve_wide_kernel<true>), grid_for(n), 256, 0, stream, kc.kc, bk, n, hj->table.as<slot_t>(), hj->mask,
+        B2_LAUNCH((retrieve_wide_kernel<true>), grid_for(n), 256, 0, stream, kc, bk, n, hj->table.as<slot_t>(), hj->mask,
                   pc.counts.as<int32_t>(), offs->data.as<int32_t>(), L->data.as<int32_t>(), R->data.as<int32_t>());
       else
-        B2_LAUNCH((retrieve_wide_kernel<false>), grid_for(n), 256, 0, stream, kc.kc, bk, n, hj->table.as<slot_t>(), hj->mask,
+        B2_LAUNCH((retrieve_wide_kernel<false>), grid_for(n), 256, 0, stream, kc, bk, n, hj->table.as<slot_t>(), hj->mask,
                   pc.counts.as<int32_t>(), offs->data.as<int32_t>(), L->data.as<int32_t>(), R->data.as<int32_t>());
     } else if (left)
       B2_LAUNCH((retrieve_kernel<true>), grid_for(n), 256, 0, stream, kc, n, hj->table.as<slot_t>(), hj->mask,
@@ -636,10 +528,7 @@ column_ptr hash_join_match_counts(const b2_hash_join* hj, const std::vector<b2_c
   const bool left = kind != JOIN_INNER;
   auto out = make_column(B2_INT32, (int32_t)n, false, stream);
   if (n == 0) return out;
-  // counts must come out in probe row order: pack the keys on the fly (no pre-partitioned key source)
-  key_src ks{};
-  ks.kc = make_key_cols(probe, hj->wide);
-  ks.mixed_shift = hj->mixed_shift;
+  const key_cols kc = make_key_cols(probe, hj->wide);
   int32_t* counts = out->data.as<int32_t>();
   if (hj->build_rows == 0 || hj->table.ptr == nullptr) {
     B2_LAUNCH(fill_i32_kernel, grid_for(n), 256, 0, stream, counts, n, left ? 1 : 0);
@@ -653,10 +542,10 @@ column_ptr hash_join_match_counts(const b2_hash_join* hj, const std::vector<b2_c
     prof_scope ps("join_count", stream);
     if (hj->wide) {
       const key_cols bk = make_key_cols(hj->build_cols, true);
-      B2_LAUNCH((count_wide_kernel<false>), grid_for(n), 256, 0, stream, ks.kc, bk, n, skip_nulls, hj->table_has_null_rows, table, hj->mask,
+      B2_LAUNCH((count_wide_kernel<false>), grid_for(n), 256, 0, stream, kc, bk, n, skip_nulls, hj->table_has_null_rows, table, hj->mask,
                 counts, tot.as<unsigned long long>());
     } else {
-      B2_LAUNCH((count_kernel<false>), grid_for(n), 256, 0, stream, ks, n, skip_nulls, hj->table_has_null_rows, table, hj->mask, counts,
+      B2_LAUNCH((count_kernel<false>), grid_for(n), 256, 0, stream, kc, n, skip_nulls, hj->table_has_null_rows, table, hj->mask, counts,
                 tot.as<unsigned long long>());
     }
   }
@@ -694,14 +583,12 @@ void hash_join_partitioned(const b2_hash_join* hj, const std::vector<b2_column_v
   out_left  = make_column(B2_INT32, (int32_t)total, false, stream);
   out_right = make_column(B2_INT32, (int32_t)total, false, stream);
   if (total == 0) return;
-  key_src ks{};
-  ks.kc = make_key_cols(probe, hj->wide);
-  ks.mixed_shift = hj->mixed_shift;
+  const key_cols pk = make_key_cols(probe, hj->wide);
   const key_cols bk = hj->wide ? make_key_cols(hj->build_cols, true) : key_cols{};
   const slot_t* table = hj->build_rows > 0 ? hj->table.as<slot_t>() : nullptr;
   prof_scope ps("join_retrieve", stream);
 #define B2_RP(L, W)                                                                                                              \
-  B2_LAUNCH((retrieve_part_kernel<L, W>), grid_for(m), 256, 0, stream, ks, bk, (int64_t)left_start, m, table, hj->mask, counts, \
+  B2_LAUNCH((retrieve_part_kernel<L, W>), grid_for(m), 256, 0, stream, pk, bk, (int64_t)left_start, m, table, hj->mask, counts, \
             offs->data.as<int32_t>(), out_left->data.as<int32_t>(), out_right->data.as<int32_t>())
   if (left) { if (hj->wide) B2_RP(true, true); else B2_RP(true, false); }
   else      { if (hj->wide) B2_RP(false, true); else B2_RP(false, false); }

@@ -1,7 +1,7 @@
 // radix_join.cu — partitioned ("radix") inner join for large null-free key tables.
 //
 // Default for cudf::inner_join / left_join / full_join calls whose two sides both have at least 2^24 rows
-// (B2_JOIN_RADIX_ROWS=<rows> moves the limit, 0 switches the path off).  Validated on hardware in round 2.
+// (B2_JOIN_RADIX_ROWS=<rows> moves the limit, 0 switches the path off).
 //
 // Same contract as the hash path it stands in for (cpp/src/join/join.cu:27-110 inner_join over
 // cpp/src/join/hash_join/hash_join.cu:32-299): all (probe row, build row) pairs with equal keys, in unspecified
@@ -100,9 +100,7 @@ __device__ __forceinline__ uint32_t rj_slot(uint64_t h) { return (uint32_t)(h >>
 // LEFT: a probe row without any match (over all build chunks) yields one pair (row, JoinNoMatch); a thread owns the same
 // <= 64 probe rows in every chunk round, so one 64-bit register remembers which of them have matched.
 constexpr int RJ_BATCH = 8;
-constexpr int RJ_DEFAULT_KERNEL = 1;
 
-template <int NTHREADS = RJ_THREADS>
 __device__ __forceinline__ unsigned long long rj_block_reserve(unsigned long long mine, unsigned long long* cursor, unsigned long long* s_wsum,
                                                                unsigned long long* s_base)
 {
@@ -117,14 +115,14 @@ __device__ __forceinline__ unsigned long long rj_block_reserve(unsigned long lon
   if (lane == 31) s_wsum[warp] = inc;
   __syncthreads();
   if (warp == 0) {
-    unsigned long long w = lane < NTHREADS / 32 ? s_wsum[lane] : 0ull;
+    unsigned long long w = lane < RJ_THREADS / 32 ? s_wsum[lane] : 0ull;
     unsigned long long winc = w;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
       const unsigned long long nb = __shfl_up_sync(0xffffffffu, winc, o);
       if (lane >= o) winc += nb;
     }
-    if (lane < NTHREADS / 32) s_wsum[lane] = winc - w;  // exclusive offset of each warp
+    if (lane < RJ_THREADS / 32) s_wsum[lane] = winc - w;  // exclusive offset of each warp
     if (lane == 31) *s_base = winc ? atomicAdd(cursor, winc) : 0ull;
   }
   __syncthreads();
@@ -242,144 +240,6 @@ rj_join_kernel(const uint64_t* __restrict__ bh, const int32_t* __restrict__ bid,
   }
 }
 
-// ---- rj2: the same walk with a tag table instead of staged keys, two CTAs per SM -------------------------------------------
-// rj_join_kernel needs 160 KB of shared memory (keys + 16-bit slots), so ONE 1024-thread CTA owns an SM and every one of its
-// ~9 barriers per item idles the whole SM. Here a slot is one 32-bit word
-// {16-bit tag = low bits of h, 15-bit local build row}; the build keys are never staged: a tag match is confirmed against
-// the key in global memory (the partition's keys were streamed by this CTA a moment ago: L2 hits, and only rows whose tag
-// matches pay it — the true matches plus 2^-16 of the other compares). 110 KB per CTA => two 512-thread CTAs per SM with
-// independent barriers; a probe step is one LDS.32 instead of LDS.U16 + LDS.64.
-// slot = mulhi(bits 16..47 of h, slots) (bits 48..63 are the partition), slots chosen per chunk (>= 2 x rows), so small
-// partitions reset and probe a small table.
-constexpr int RJ2_THREADS = 512;
-constexpr int RJ2_SLOTS   = 28160;             // 110 KB of 32-bit slots
-constexpr int RJ2_CAP     = 16896;             // build rows per chunk: load factor <= 0.6; row numbers fit 15 bits
-constexpr int RJ2_PIECE   = 64 * RJ2_THREADS;  // probe rows per work item (one bit per row of a thread)
-constexpr size_t RJ2_SMEM = (size_t)RJ2_SLOTS * sizeof(uint32_t);
-constexpr uint32_t RJ2_EMPTY = 0xFFFFFFFFu;
-static_assert(RJ2_CAP < 32768, "local build rows are stored in 15 bits (bit 15 stays clear: no entry equals RJ2_EMPTY)");
-
-__device__ __forceinline__ uint32_t rj2_slot(uint64_t h, uint32_t slots) { return __umulhi((uint32_t)(h >> 16), slots); }
-
-template <bool LEFT = false>
-__global__ void __launch_bounds__(RJ2_THREADS, 2)
-rj2_join_kernel(const uint64_t* __restrict__ bh, const int32_t* __restrict__ bid, const int32_t* __restrict__ boff,
-                const uint64_t* __restrict__ ph, const int32_t* __restrict__ pid, const int32_t* __restrict__ poff,
-                const int32_t* __restrict__ item_first, const int32_t* __restrict__ item_part, unsigned long long* __restrict__ cursor,
-                unsigned long long capacity, int32_t* __restrict__ out_probe, int32_t* __restrict__ out_build)
-{
-  B2_DYNAMIC_SMEM(rj_smem);
-  uint32_t* tab = reinterpret_cast<uint32_t*>(rj_smem);
-  __shared__ unsigned long long s_wsum[RJ2_THREADS / 32];
-  __shared__ unsigned long long s_base;
-
-  const int item = blockIdx.x;
-  const int tid  = threadIdx.x;
-  if (item >= item_first[RJ_PARTS]) return;  // the grid is sized for the worst case; uniform over the CTA
-  const int part = item_part[item];
-  const int b0 = boff[part], b1 = boff[part + 1];
-  const int64_t p0 = (int64_t)poff[part] + (int64_t)(item - item_first[part]) * RJ2_PIECE;
-  const int64_t p1 = min(p0 + RJ2_PIECE, (int64_t)poff[part + 1]);
-  constexpr int ROUNDS = RJ2_PIECE / RJ2_THREADS;
-  static_assert(ROUNDS <= 64 && ROUNDS % RJ_BATCH == 0, "one bit per probe row of a thread; whole batches");
-  const int my_rounds = (int)((p1 - p0 - tid + RJ2_THREADS - 1) / RJ2_THREADS);  // rows p0 + tid + k * RJ2_THREADS, k < my_rounds (may be <= 0)
-  unsigned long long matched = 0;
-  for (int64_t c0 = b0; c0 < b1; c0 += RJ2_CAP) {
-    const int cn = (int)min((int64_t)RJ2_CAP, (int64_t)b1 - c0);
-    const uint32_t slots = (uint32_t)min(RJ2_SLOTS, max(1024, (cn * 2 + 1023) & ~1023));
-    const uint64_t* __restrict__ bkeys = bh + c0;
-    __syncthreads();  // the previous chunk's probes are done before the table is reset
-    for (uint32_t i = tid; i < slots; i += RJ2_THREADS) tab[i] = RJ2_EMPTY;
-    __syncthreads();
-    // insert: batches of build keys straight from global memory; one CAS per visited slot
-    for (int jb = tid; jb < cn; jb += RJ_BATCH * RJ2_THREADS) {
-      uint64_t h[RJ_BATCH];
-#pragma unroll
-      for (int u = 0; u < RJ_BATCH; ++u) h[u] = (jb + u * RJ2_THREADS < cn) ? ld_stream(bkeys + jb + u * RJ2_THREADS) : 0ull;
-#pragma unroll
-      for (int u = 0; u < RJ_BATCH; ++u) {
-        const int j = jb + u * RJ2_THREADS;
-        if (j >= cn) break;
-        const uint32_t w = ((uint32_t)(h[u] & 0xFFFFull) << 16) | (uint32_t)j;
-        uint32_t s = rj2_slot(h[u], slots);
-        while (atomicCAS(&tab[s], RJ2_EMPTY, w) != RJ2_EMPTY) s = (s + 1 == slots) ? 0u : s + 1;
-      }
-    }
-    __syncthreads();
-    // ---- walk 1: count this chunk's matches, remember which of my rows matched ----
-    unsigned long long hit = 0, local = 0;
-    for (int kb = 0; kb < ROUNDS; kb += RJ_BATCH) {
-      if (kb >= my_rounds) break;
-      uint64_t h[RJ_BATCH];
-#pragma unroll
-      for (int u = 0; u < RJ_BATCH; ++u) h[u] = (kb + u < my_rounds) ? ld_stream(ph + p0 + tid + (int64_t)(kb + u) * RJ2_THREADS) : 0ull;
-#pragma unroll
-      for (int u = 0; u < RJ_BATCH; ++u) {
-        if (kb + u >= my_rounds) break;
-        const uint32_t tag = (uint32_t)(h[u] & 0xFFFFull);
-        uint32_t s = rj2_slot(h[u], slots);
-        while (true) {
-          const uint32_t e = tab[s];
-          if (e == RJ2_EMPTY) break;
-          if ((e >> 16) == tag && bkeys[e & 0x7FFFu] == h[u]) {
-            ++local;
-            hit |= 1ull << (kb + u);
-          }
-          s = (s + 1 == slots) ? 0u : s + 1;
-        }
-      }
-    }
-    if (LEFT) matched |= hit;
-    // ---- one reservation for the chunk, then walk 2 over the rows that matched ----
-    unsigned long long pos = rj_block_reserve<RJ2_THREADS>(local, cursor, s_wsum, &s_base);
-    while (hit) {
-      const int k = (uint32_t)hit ? __ffs((int)(uint32_t)hit) - 1 : 32 + __ffs((int)(uint32_t)(hit >> 32)) - 1;
-      hit &= hit - 1;
-      const int64_t i = p0 + tid + (int64_t)k * RJ2_THREADS;
-      const uint64_t h = ph[i];
-      const int32_t prow = pid[i];
-      const uint32_t tag = (uint32_t)(h & 0xFFFFull);
-      uint32_t s = rj2_slot(h, slots);
-      while (true) {
-        const uint32_t e = tab[s];
-        if (e == RJ2_EMPTY) break;
-        if ((e >> 16) == tag && bkeys[e & 0x7FFFu] == h) {
-          if (pos < capacity) {
-            out_probe[pos] = prow;
-            out_build[pos] = bid[c0 + (e & 0x7FFFu)];
-          }
-          ++pos;
-        }
-        s = (s + 1 == slots) ? 0u : s + 1;
-      }
-    }
-  }
-  if (LEFT) {
-    unsigned long long un = 0;  // my rows that never matched
-    for (int k = 0; k < my_rounds; ++k) un += ((matched >> k) & 1ull) ? 0ull : 1ull;
-    unsigned long long pos = rj_block_reserve<RJ2_THREADS>(un, cursor, s_wsum, &s_base);
-    for (int k = 0; k < my_rounds; ++k) {
-      if ((matched >> k) & 1ull) continue;
-      if (pos < capacity) {
-        out_probe[pos] = pid[p0 + tid + (int64_t)k * RJ2_THREADS];
-        out_build[pos] = B2_JOIN_NO_MATCH;
-      }
-      ++pos;
-    }
-  }
-}
-
-// B2_JOIN_KERNEL=1: rj_join_kernel (keys staged in shared memory, one 1024-thread CTA per SM); 2: rj2_join_kernel
-int rj_kernel_choice()
-{
-  static const int v = [] {
-    const char* e = std::getenv("B2_JOIN_KERNEL");
-    const int k = e ? std::atoi(e) : 0;
-    return (k == 1 || k == 2) ? k : RJ_DEFAULT_KERNEL;
-  }();
-  return v;
-}
-
 bool any_nulls(const std::vector<b2_column_view>& cols)
 {
   for (auto& c : cols)
@@ -440,21 +300,17 @@ void radix_join(const std::vector<b2_column_view>& build, const std::vector<b2_c
   once_per_device(attr_done, [] {
     B2_CUDA_TRY(cudaFuncSetAttribute(rj_join_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RJ_SMEM));
     B2_CUDA_TRY(cudaFuncSetAttribute(rj_join_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RJ_SMEM));
-    B2_CUDA_TRY(cudaFuncSetAttribute(rj2_join_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RJ2_SMEM));
-    B2_CUDA_TRY(cudaFuncSetAttribute(rj2_join_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)RJ2_SMEM));
   });
-  const bool tagged = rj_kernel_choice() == 2;
-  const int piece = tagged ? RJ2_PIECE : RJ_PIECE;
   rj_side bs, ps;
   rj_partition(build, stream, bs);
   rj_partition(probe, stream, ps);
 
-  // work items: (partition, piece of <= `piece` probe rows); at most RJ_PARTS + n_probe / piece of them
+  // work items: (partition, piece of <= RJ_PIECE probe rows); at most RJ_PARTS + n_probe / RJ_PIECE of them
   const int64_t n_probe = probe[0].size;
-  const int32_t max_items = (int32_t)(RJ_PARTS + n_probe / piece + 1);
+  const int32_t max_items = (int32_t)(RJ_PARTS + n_probe / RJ_PIECE + 1);
   dbuf pieces(sizeof(int32_t) * (RJ_PARTS + 1), stream);
   B2_LAUNCH(rj_pieces_kernel, (RJ_PARTS + 1 + 255) / 256, 256, 0, stream, bs.off.as<int32_t>(), ps.off.as<int32_t>(), left, pieces.as<int32_t>(),
-            piece);
+            RJ_PIECE);
   b2_column_view pv{B2_INT32, (int32_t)(RJ_PARTS + 1), pieces.ptr, nullptr, 0, 0};
   auto item_first = scan(pv, B2_AGG_SUM, B2_SCAN_EXCLUSIVE, B2_NULL_EXCLUDE, stream);
 
@@ -477,18 +333,8 @@ void radix_join(const std::vector<b2_column_view>& build, const std::vector<b2_c
                            bs.off.as<int32_t>(), ps.h.as<uint64_t>(), ps.ids.as<int32_t>(), ps.off.as<int32_t>(),                        \
                            item_first->data.as<int32_t>(), item_part.as<int32_t>(), tot.as<unsigned long long>(), capacity, op->data.as<int32_t>(),   \
                            ob->data.as<int32_t>())
-#define B2_RJ2(L) B2_LAUNCH((rj2_join_kernel<L>), max_items, RJ2_THREADS, RJ2_SMEM, stream, bs.h.as<uint64_t>(), bs.ids.as<int32_t>(),   \
-                            bs.off.as<int32_t>(), ps.h.as<uint64_t>(), ps.ids.as<int32_t>(), ps.off.as<int32_t>(),                       \
-                            item_first->data.as<int32_t>(), item_part.as<int32_t>(), tot.as<unsigned long long>(), capacity, op->data.as<int32_t>(),  \
-                            ob->data.as<int32_t>())
-      if (tagged) {
-        if (left) B2_RJ2(true);
-        else B2_RJ2(false);
-      } else {
-        if (left) B2_RJ(true);
-        else B2_RJ(false);
-      }
-#undef B2_RJ2
+      if (left) B2_RJ(true);
+      else B2_RJ(false);
 #undef B2_RJ
     }
     unsigned long long m = 0;

@@ -1656,20 +1656,17 @@ void run_radix(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int32_t
   run_radix_cfg<UK, key_tile<UK>>(raw_keys, bufA, bufB, idx_out, idx_tmp, idx_tmp2, pre_idx_buf, n, kind, descending, pairs, stream);
 }
 
+// The 64-bit key kernels are instantiated here, ahead of the narrower key types that the sort entry points below instantiate.
+// How nvcc inlines the device helpers shared by the histogram, finalize and gather kernels depends on the order in which the
+// kernels are instantiated; this order gives every kernel the code the sort was measured with.
+template void run_radix_cfg<uint64_t, tile_384x16>(const uint64_t*, uint64_t*, uint64_t*, int32_t*, int32_t*, int32_t*, int, int64_t, int, bool,
+                                                   bool, cudaStream_t, int, int, bool, const void*, uint32_t*);
+
 }  // namespace
 
-// Stable partial sort of n 64-bit keys by their two most significant bytes (passes 6 and 7 only):
-// keys_out / idx_out receive the keys and their original positions grouped by the 16-bit prefix.
-// Used by the hash join to make build and probe walk the table region by region (L2 locality).
-void radix_partition_top16(const uint64_t* keys_in, int64_t n, uint64_t* keys_out, int32_t* idx_out, cudaStream_t stream)
-{
-  dbuf b(sizeof(uint64_t) * n, stream), it(sizeof(int32_t) * n, stream);
-  run_radix_cfg<uint64_t, tile_384x16>(keys_in, keys_out, b.as<uint64_t>(), idx_out, it.as<int32_t>(), nullptr, 0, n,
-                                       (int)key_kind::UNSIGNED, false, true, stream, 6, 7, true);
-}
-
-// Same, but `packed_keys` are the raw packed join keys: the kernels apply mix64 on load (histogram of the two
-// needed digits only), so keys_out receives mix64(key) grouped by its top 16 bits. Used by the partitioned join (radix_join.cu).
+// Stable partial sort of n 64-bit packed join keys by the two most significant bytes of mix64(key) (passes 6 and 7
+// only): the kernels apply mix64 on load (histogram of the two needed digits only), so keys_out / idx_out receive
+// mix64(key) and the original positions grouped by its top 16 bits. Used by the partitioned join (radix_join.cu).
 void radix_partition_top16_mix(const uint64_t* packed_keys, int64_t n, uint64_t* keys_out, int32_t* idx_out, cudaStream_t stream)
 {
   dbuf b(sizeof(uint64_t) * n, stream), it(sizeof(int32_t) * n, stream);

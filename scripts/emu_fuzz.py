@@ -15,9 +15,7 @@ sys.path.insert(0, ROOT)
 os.chdir(ROOT)
 
 # --mode selects an opt-in path for the whole run (the switches are read by the library, some of them only once)
-_MODES = {"default": {}, "carry": {"B2_SORT_CARRY": "1"}, "alias": {"B2_SORT_ALIAS": "1"}, "radix": {"B2_JOIN_RADIX_ROWS": "1"},
-          "portion": {"B2_SORT_PORTION": "6144"}, "mixed": {"B2_JOIN_PARTITION_ROWS": "64"},
-          "radix2": {"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_KERNEL": "2"},
+_MODES = {"default": {}, "carry": {"B2_SORT_CARRY": "1"}, "radix": {"B2_JOIN_RADIX_ROWS": "1"}, "portion": {"B2_SORT_PORTION": "6144"},
           "pgb": {"B2_GROUPBY_PARTITION_ROWS": "1", "B2_GROUPBY_EST": "1", "B2_GROUPBY_EST_MIN": "1"},
           "pgbcap": {"B2_GROUPBY_PARTITION_ROWS": "1", "B2_GROUPBY_EST": "1", "B2_GROUPBY_EST_MIN": "1", "B2_GROUPBY_EST_CAP": "48"},
           "pgbhist": {"B2_GROUPBY_PARTITION_ROWS": "1", "B2_GROUPBY_EST": "0"},

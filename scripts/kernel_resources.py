@@ -8,7 +8,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 LIB = ROOT / "cudf_b200" / "libcudf_b200.so"
-INTEREST = ["onesweep_kernel", "histogram_kernel", "segment_fix_kernel", "plan_kernel", "rj_join_kernel", "rj2_join_kernel", "pgb_agg_kernel",
+INTEREST = ["onesweep_kernel", "histogram_kernel", "segment_fix_kernel", "plan_kernel", "rj_join_kernel", "pgb_agg_kernel",
             "scan_kernel", "reduce_kernel", "segreduce_kernel", "gather_kernel", "range_count_kernel", "build_kernel", "groupby_kernel",
             "compact_kernel", "scatter_staged_kernel", "peer_copy_kernel"]
 

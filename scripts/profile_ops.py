@@ -1,7 +1,6 @@
 """Small driver for ncu captures of one operation (after one warm-up call):
   python scripts/profile_ops.py --op sort_by_key|sort|inner_join|groupby|scan [--rows N]
-Opt-in paths are selected with their environment switches (README), e.g. B2_SORT_ALIAS=1, B2_SORT_CARRY=1,
-B2_JOIN_RADIX_ROWS=1."""
+Other paths are selected with their environment switches (README), e.g. B2_SORT_CARRY=0, B2_JOIN_RADIX_ROWS=1."""
 import argparse
 import ctypes as C
 import sys

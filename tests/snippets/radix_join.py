@@ -1,21 +1,20 @@
-"""Shared body of the checks of the partitioned join (radix_join.cu: rj_join_kernel, and rj2_join_kernel with
-B2_JOIN_KERNEL=2) at the constants where its index arithmetic can go wrong. Run by tests/test_emu_join_radix.py on the CPU
+"""Shared body of the checks of the partitioned join (radix_join.cu: rj_join_kernel) at the constants where its index
+arithmetic can go wrong. Run by tests/test_emu_join_radix.py on the CPU
 emulator and by tests/test_join_radix_gpu.py on the GPU, both with B2_JOIN_RADIX_ROWS=1 so that small inputs take the
 path. `plc`, `np`, `ojoin`, `L` are provided by the caller; FULL = False drops the slowest sizes of a case (the emulator).
 
 The keys are built from the value the kernels work on: h = mix64(packed key) is a bijection, so a case picks h and uses
-unmix64(h) as its key. The partition of a row is h >> 48; rj_join_kernel's slot is bits 33..47 of h; rj2_join_kernel's tag is
-h & 0xFFFF and its slot is mulhi(bits 16..47 of h, slots). Within a partition both sides keep their input order (the
-partition passes are stable), so a case also decides which build chunk and which probe piece a row lands in.
+unmix64(h) as its key. The partition of a row is h >> 48 and its slot is bits 33..47 of h. Within a partition both sides
+keep their input order (the partition passes are stable), so a case also decides which build chunk and which probe piece a
+row lands in.
 
 Which path ran is read from the profiling scopes: radix_join opens one `rjoin_join` scope per walk, so a call that took the
 hash table shows 0, a normal call 1 and a call whose output outgrew the size guess (and walked again) 2."""
 HELPERS = r"""
 import os
 rng = np.random.default_rng(2024)
-KERNEL = int(os.environ.get('B2_JOIN_KERNEL', '1'))
-CAP = 16384 if KERNEL == 1 else 16896      # build rows per shared-memory chunk (RJ_CAP / RJ2_CAP)
-PIECE = 65536 if KERNEL == 1 else 32768    # probe rows per work item (RJ_PIECE / RJ2_PIECE): 64 rows per thread
+CAP = 16384      # build rows per shared-memory chunk (RJ_CAP)
+PIECE = 65536    # probe rows per work item (RJ_PIECE): 64 rows per thread
 U = np.uint64
 
 def mix64(k):
@@ -37,12 +36,6 @@ assert np.array_equal(mix64(unmix64(_t)), _t) and np.array_equal(unmix64(mix64(_
 
 def k1_slot(h):
     return (h >> U(33)) & U(32767)
-
-def k2_slots(cn):
-    return min(28160, max(1024, (cn * 2 + 1023) & ~1023))
-
-def k2_slot(h, slots):
-    return (((h >> U(16)) & U(0xFFFFFFFF)) * U(slots)) >> U(32)
 
 def f64_ok(h):
     # the key bits must survive the float64 normalisation unchanged: no NaN, no -0.0
@@ -127,13 +120,12 @@ for i, nb in enumerate((CAP, CAP + 1, 2 * CAP, 2 * CAP + 1) if FULL else (CAP + 
     form = FORMS[i % 3]
     check(cols(p, form), cols(b, form), ALL, 1)
 
-# ---- the 32768-slot table wraps: ~3000 build keys of one partition all in slot 32767 (rj2: the last slot too) ----
+# ---- the 32768-slot table wraps: ~3000 build keys of one partition all in slot 32767 ----
 CASE = 'slot wrap'
 P = 0x4321
 W = 3000 if FULL else 400
 h = draw(W + W // 3, P, low_bits=33, fixed=32767 << 33)
 assert (k1_slot(h) == 32767).all() and (h >> U(48) == P).all()
-assert (k2_slot(h[:W], k2_slots(W)) == k2_slots(W) - 1).all()
 bh, absent = h[:W], h[W:]
 p = rng.permutation(np.concatenate([bh, absent, bh[:W // 2]]))
 check(cols(p, 'i64'), cols(bh, 'i64'), ('inner_join', 'left_join'), 1)
@@ -162,26 +154,6 @@ check(cols(p, 'i64'), cols(b, 'i64'), ALL, 1)
 CASE = 'probe partition without build rows'
 check(cols(h1, 'i64'), cols(h0[:300], 'i64'), ALL, 1)
 check(cols(h0, 'f64'), cols(h1[:300], 'f64'), ALL, 1)
-
-# ---- rj2: equal tag and slot but different keys; table sizes rounded to 1024 slots; the wrap at s + 1 == slots ----
-P = 0x0777
-for nb in (511, 512, 513):
-    CASE = f'tags and small tables nb={nb}'
-    slots = k2_slots(nb)
-    base = draw(4 * nb, P, low_bits=47)              # bits 16..47 below all-ones: h + (1 << 16) stays in the partition
-    twin = base + U(1 << 16)                         # same tag (low 16 bits), next value of bits 16..47
-    ok = (k2_slot(base, slots) == k2_slot(twin, slots)) & f64_ok(twin) & ~np.isin(twin, base)
-    base, twin = base[ok], twin[ok]
-    assert len(base) >= nb + 100
-    last = draw(12, P, low_bits=16, fixed=(0xFFFFFFFF - 7) << 16)  # bits 16..47 near all-ones: the last slot
-    assert (k2_slot(last, slots) == slots - 1).all()
-    nt = 40
-    bh = np.concatenate([base[:nb - nt - len(last)], twin[:nt], last])      # rows 0..nt-1 of base and twin both built
-    assert len(bh) == nb and len(np.unique(bh)) == nb
-    lone = twin[nt:2 * nt]                                                     # twins of built keys, absent themselves
-    assert np.isin(base[nt:2 * nt], bh).all() and not np.isin(lone, bh).any()
-    p = rng.permutation(np.concatenate([bh, lone, lone, base[nb:nb + 100]]))
-    check(cols(p, 'i64'), cols(bh, 'i64'), ALL, 1)
 
 # ---- key types through rj_pack_kernel: pack_row's normalisation against the oracle's row equality ----
 # The right (build) side holds each key at most once, so no call outgrows the one-pair-per-probe-row guess.

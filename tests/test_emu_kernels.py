@@ -42,7 +42,7 @@ def emu_lib():
 
 def run(code: str, marker: str, env=None, timeout=900):
     e = dict(os.environ)
-    for k in ("B2_JOIN_RADIX_CAPACITY", "B2_SORT_PLAN_READBACK_MIN", "B2_GROUPBY_PARTITION_ROWS", "B2_GROUPBY_SMEM_SLOTS", "B2_SORT_HYBRID", "B2_SORT_HYBRID_MIN", "B2_SORT_FIX_FAST", "B2_SORT_CARRY", "B2_SORT_ALIAS", "B2_JOIN_RADIX_ROWS", "B2_JOIN_KERNEL", "B2_GROUPBY_EST", "B2_GROUPBY_EST_MIN", "B2_GROUPBY_EST_CAP", "B2_JOIN_PARTITION_ROWS", "B2_SORT_PORTION"):
+    for k in ("B2_JOIN_RADIX_CAPACITY", "B2_SORT_PLAN_READBACK_MIN", "B2_GROUPBY_PARTITION_ROWS", "B2_GROUPBY_SMEM_SLOTS", "B2_SORT_HYBRID", "B2_SORT_HYBRID_MIN", "B2_SORT_FIX_FAST", "B2_SORT_CARRY", "B2_JOIN_RADIX_ROWS", "B2_GROUPBY_EST", "B2_GROUPBY_EST_MIN", "B2_GROUPBY_EST_CAP", "B2_SORT_PORTION"):
         e.pop(k, None)
     e.update(env or {})
     r = subprocess.run([sys.executable, "-c", PRELUDE + code], capture_output=True, text=True, env=e, cwd=ROOT, timeout=timeout)
@@ -123,7 +123,8 @@ def test_emu_groupby_partitioned(emu_lib):
         run(cases + CODE, "PGB_OK", env=dict(env, B2_GROUPBY_PARTITION_ROWS="1"))
 
 
-def test_emu_sort_alias(emu_lib):
+def test_emu_sort_by_key_aliased_column(emu_lib):
+    """sort_by_key(T, T): the values and the keys are the same column."""
     run(r"""
 rng = np.random.default_rng(11)
 for n in (1, 33, 6145, 20_003):
@@ -135,7 +136,7 @@ for n in (1, 33, 6145, 20_003):
             exp = np.sort(keys, kind='stable')
             assert np.array_equal(got, exp[::-1] if order else exp), (n, dt, order)
 print('ALIAS_OK')
-""", "ALIAS_OK", env={"B2_SORT_ALIAS": "1"})
+""", "ALIAS_OK")
 
 
 def test_emu_radix_inner_join(emu_lib):
@@ -165,16 +166,10 @@ b = rng.integers(0, 100_000, 40_000); b[:20_000] = 555
 check([(p[:DUPN], None)], [(b, None)], 'dup x chunks', ("inner_join", "left_join"))
 print('RADIX_JOIN_OK')
 """
-    run("DUPN = 600\n" + code, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_KERNEL": "1"})
-    # the tag-table kernel (two CTAs per SM): without the two slowest cases of the emulation (their work-item logic is shared)
-    a, b = code.index("b = rng.integers(0, 1000, 60_000)"), code.index("# packed two-column float key")
-    c, d = code.index("# probe-side hot key"), code.index("# a left join whose hot probe key")
-    lighter = code[:a] + code[b:c] + code[d:]
-    run("DUPN = 400\n" + lighter, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_KERNEL": "2"})
+    run("DUPN = 600\n" + code, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1"})
     # output-size guess too small: the walk is repeated with the exact size (first case only: the emulator is slow)
     short = code[:code.index("check([(rng.integers(0, 90_000, 7_000)")] + "print('RADIX_JOIN_OK')\n"
-    run(short, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_RADIX_CAPACITY": "100", "B2_JOIN_KERNEL": "1"})
-    run(short, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_RADIX_CAPACITY": "100", "B2_JOIN_KERNEL": "2"})
+    run(short, "RADIX_JOIN_OK", env={"B2_JOIN_RADIX_ROWS": "1", "B2_JOIN_RADIX_CAPACITY": "100"})
 
 
 def test_emu_wide_keys(emu_lib):

@@ -1,9 +1,8 @@
 """The partitioned join (radix_join.cu) on the GPU.
 
-test_radix_join_cases runs tests/snippets/radix_join.py with B2_JOIN_RADIX_ROWS=1, once per join kernel (B2_JOIN_KERNEL is
-read once per process): keys built from their mixed hash so that they land on the chunk, slot, piece, partition and tag
-boundaries of the kernels, key types through the pack kernel, sliced views, the output-size rerun, and the conditions that
-send a join to the hash table. test_radix_join_switch_point checks, with no switches set, that 2^24 rows on both sides take the
+test_radix_join_cases runs tests/snippets/radix_join.py with B2_JOIN_RADIX_ROWS=1: keys built from their mixed hash so that
+they land on the chunk, slot, piece and partition boundaries of the join kernel, key types through the pack kernel, sliced
+views, the output-size rerun, and the conditions that send a join to the hash table. test_radix_join_switch_point checks, with no switches set, that 2^24 rows on both sides take the
 path and 2^24 - 1 rows on one side do not."""
 import os
 import subprocess
@@ -23,7 +22,7 @@ from cudf_b200 import _lib as L
 from oracle import join as ojoin
 """
 
-SWITCHES = ("B2_JOIN_RADIX_ROWS", "B2_JOIN_RADIX_CAPACITY", "B2_JOIN_KERNEL", "B2_SORT_PORTION", "B2_JOIN_PARTITION_ROWS")
+SWITCHES = ("B2_JOIN_RADIX_ROWS", "B2_JOIN_RADIX_CAPACITY", "B2_SORT_PORTION")
 
 
 def _run(code, marker, **env):
@@ -33,11 +32,10 @@ def _run(code, marker, **env):
     assert marker in r.stdout and r.returncode == 0, r.stdout[-1500:] + r.stderr[-2500:]
 
 
-@pytest.mark.parametrize("kernel", ["1", "2"])
-def test_radix_join_cases(kernel):
+def test_radix_join_cases():
     from tests.snippets.radix_join import CODE
 
-    _run("FULL = True\n" + CODE, "RADIX_JOIN_CASES_OK", B2_JOIN_RADIX_ROWS="1", B2_JOIN_KERNEL=kernel)
+    _run("FULL = True\n" + CODE, "RADIX_JOIN_CASES_OK", B2_JOIN_RADIX_ROWS="1")
 
 
 def test_radix_join_portions():

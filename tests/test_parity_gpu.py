@@ -423,36 +423,22 @@ def test_partition(plc):
     assert res.columns()[1].null_count() == int((~valid).sum())
 
 
-def test_join_partitioned_path_small():
-    """The mixed-key / radix-partitioned join path (normally >= 4M rows) forced on small inputs."""
-    import os
-    import subprocess
-    import sys
-
-    code = r"""
-import numpy as np, sys
-sys.path.insert(0, '.')
-import cudf_b200.pylibcudf as plc
-from oracle import join as ojoin
-from tests.impls import PlcImpl
-cu = PlcImpl(plc)
-rng = np.random.default_rng(77)
-for dtype in (np.int64, np.int32, np.float64, np.int8):
-    for nl, nr in [(1000, 700), (50_000, 20_000), (300, 90_000)]:
-        hi = 100 if dtype == np.int8 else 5000
-        l = [(rng.integers(0, hi, nl).astype(dtype), rng.random(nl) < 0.9 if dtype == np.int32 else None)]
-        r = [(rng.integers(0, hi, nr).astype(dtype), None)]
-        for kind in ("inner_join", "left_join", "full_join"):
-            for ne in (0, 1):
-                got = getattr(cu, kind)(l, r, ne)
-                exp = getattr(ojoin, kind)(l, r, ne)
-                assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (dtype, nl, nr, kind, ne)
-l = [(rng.integers(0, 50, 20000).astype(np.int32), None), (rng.integers(0, 9, 20000).astype(np.int16), None)]
-r = [(rng.integers(0, 50, 9000).astype(np.int32), None), (rng.integers(0, 9, 9000).astype(np.int16), None)]
-got = cu.inner_join(l, r); exp = ojoin.inner_join(l, r)
-assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1])
-print('PARTITIONED_JOIN_OK')
-"""
-    env = dict(os.environ, B2_JOIN_PARTITION_ROWS="64")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, cwd=os.path.dirname(os.path.dirname(__file__)))
-    assert "PARTITIONED_JOIN_OK" in r.stdout, r.stdout[-2000:] + r.stderr[-3000:]
+def test_join_hash_table_small(cu):
+    """Inner / left / full joins on the hash table: one key column of four types (int32 with nulls) at three size ratios
+    under both null equalities, and a packed int32 + int16 key."""
+    rng = np.random.default_rng(77)
+    for dtype in (np.int64, np.int32, np.float64, np.int8):
+        for nl, nr in [(1000, 700), (50_000, 20_000), (300, 90_000)]:
+            hi = 100 if dtype == np.int8 else 5000
+            l = [(rng.integers(0, hi, nl).astype(dtype), rng.random(nl) < 0.9 if dtype == np.int32 else None)]
+            r = [(rng.integers(0, hi, nr).astype(dtype), None)]
+            for kind in ("inner_join", "left_join", "full_join"):
+                for ne in (0, 1):
+                    got = getattr(cu, kind)(l, r, ne)
+                    exp = getattr(ojoin, kind)(l, r, ne)
+                    assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1]), (dtype, nl, nr, kind, ne)
+    l = [(rng.integers(0, 50, 20000).astype(np.int32), None), (rng.integers(0, 9, 20000).astype(np.int16), None)]
+    r = [(rng.integers(0, 50, 9000).astype(np.int32), None), (rng.integers(0, 9, 9000).astype(np.int16), None)]
+    got = cu.inner_join(l, r)
+    exp = ojoin.inner_join(l, r)
+    assert np.array_equal(got[0], exp[0]) and np.array_equal(got[1], exp[1])

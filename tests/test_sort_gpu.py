@@ -185,6 +185,21 @@ def test_sort_by_key_carry_payload(plc):
                     assert np.array_equal(got.columns()[0].to_numpy()[0], exp), (n, kdt, vdt, order)
 
 
+def test_sort_by_key_aliased_column(plc):
+    """sort_by_key(T, T): the values and the keys are the same column."""
+    rng = np.random.default_rng(11)
+    for n in (1, 33, 6145, 200_003, 3_000_001):
+        for dt in (np.int64, np.int32, np.uint16, np.int8, np.uint64):
+            keys = rng.integers(np.iinfo(dt).min, np.iinfo(dt).max, n, dtype=dt, endpoint=True)
+            for order in (0, 1):
+                c = plc.Column.from_numpy(keys)
+                got = plc.sorting.sort_by_key(plc.Table([c]), plc.Table([c]), [order], []).columns()[0].to_numpy()[0]
+                exp = np.sort(keys, kind="stable")
+                if order == 1:
+                    exp = exp[::-1]
+                assert np.array_equal(got, exp), (n, dt, order)
+
+
 def test_sortedness_property_large(plc):
     """Size-independent properties at 2^26 rows: permutation, non-decreasing keys, stable ties."""
     import torch

@@ -32,6 +32,15 @@ class TypeId(enum.IntEnum):
     DURATION_MILLISECONDS = 19
     DURATION_MICROSECONDS = 20
     DURATION_NANOSECONDS = 21
+    # not fixed-width: no column of these types exists here; operations reject them
+    DICTIONARY32 = 22
+    STRING = 23
+    LIST = 24
+    DECIMAL32 = 25
+    DECIMAL64 = 26
+    DECIMAL128 = 27
+    STRUCT = 28
+    NUM_TYPE_IDS = 29
 
 
 class Order(enum.IntEnum):

@@ -487,6 +487,46 @@ def distinct_indices(Table input, keep, nulls_equal, nans_equal, stream=None, mr
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# binary operations (python/pylibcudf/pylibcudf/binaryop.pyx; cpp/include/cudf/binaryop.hpp)
+# ---------------------------------------------------------------------------------------------------------------------
+def binary_operation(lhs, rhs, op, output_type, stream=None, mr=None):
+    """op(lhs[i], rhs[i]) as a Column of `output_type`; each operand a Column or a Scalar, at least one a Column."""
+    cdef int32_t o = int(op)
+    cdef int32_t t = int(output_type.id())
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    cdef Column lc
+    cdef Column rc
+    cdef const b2_scalar* sc
+    if isinstance(lhs, Column) and isinstance(rhs, Column):
+        lc, rc = lhs, rhs
+        with nogil:
+            st = b2_binary_operation(&lc.v, &rc.v, o, t, s, &out)
+    elif isinstance(lhs, Column) and isinstance(rhs, _PlcScalar):
+        lc = lhs
+        sc = <const b2_scalar*><uintptr_t>rhs._handle
+        with nogil:
+            st = b2_binary_operation_cs(&lc.v, sc, o, t, s, &out)
+    elif isinstance(lhs, _PlcScalar) and isinstance(rhs, Column):
+        rc = rhs
+        sc = <const b2_scalar*><uintptr_t>lhs._handle
+        with nogil:
+            st = b2_binary_operation_sc(sc, &rc.v, o, t, s, &out)
+    else:
+        raise ValueError("binary_operation: at least one operand must be a Column, and both a Column or a Scalar")
+    check(st)
+    return Column.from_handle(out)
+
+
+def is_supported_operation(out, lhs, rhs, op):
+    """Whether binary_operation accepts these types for `op` (cudf::binops::is_supported_operation)."""
+    cdef int32_t r = 0
+    check(b2_binary_is_supported_operation(int(out.id()), int(lhs.id()), int(rhs.id()), int(op), &r))
+    return r != 0
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # joins (python/pylibcudf/pylibcudf/join.pyx:63-205; cudf::hash_join)
 # ---------------------------------------------------------------------------------------------------------------------
 ctypedef b2_status (*free_join_fn)(const b2_table_view*, const b2_table_view*, int32_t, b2_stream, b2_column**, b2_column**) noexcept nogil

@@ -156,6 +156,15 @@ cdef extern from "cudf_b200.h" nogil:
     b2_status b2_distinct_indices(const b2_table_view* input, int32_t keep, int32_t nulls_equal, int32_t nans_equal,
                                   b2_stream stream, b2_column** out)
 
+    # binary operations (cpp/include/cudf/binaryop.hpp)
+    b2_status b2_binary_operation(const b2_column_view* lhs, const b2_column_view* rhs, int32_t op, int32_t out_type, b2_stream stream,
+                                  b2_column** out)
+    b2_status b2_binary_operation_cs(const b2_column_view* lhs, const b2_scalar* rhs, int32_t op, int32_t out_type, b2_stream stream,
+                                     b2_column** out)
+    b2_status b2_binary_operation_sc(const b2_scalar* lhs, const b2_column_view* rhs, int32_t op, int32_t out_type, b2_stream stream,
+                                     b2_column** out)
+    b2_status b2_binary_is_supported_operation(int32_t out_type, int32_t lhs_type, int32_t rhs_type, int32_t op, int32_t* result)
+
     # cudf::pack / unpack (cpp/include/cudf/contiguous_split.hpp:233-317)
     void* b2_buffer_data(const b2_buffer* buf)
     size_t b2_buffer_size(const b2_buffer* buf)

@@ -113,7 +113,8 @@ constexpr size_type JoinNoMatch = INT32_MIN;
 enum class type_id : int32_t {
   EMPTY, INT8, INT16, INT32, INT64, UINT8, UINT16, UINT32, UINT64, FLOAT32, FLOAT64, BOOL8,
   TIMESTAMP_DAYS, TIMESTAMP_SECONDS, TIMESTAMP_MILLISECONDS, TIMESTAMP_MICROSECONDS, TIMESTAMP_NANOSECONDS,
-  DURATION_DAYS, DURATION_SECONDS, DURATION_MILLISECONDS, DURATION_MICROSECONDS, DURATION_NANOSECONDS
+  DURATION_DAYS, DURATION_SECONDS, DURATION_MILLISECONDS, DURATION_MICROSECONDS, DURATION_NANOSECONDS,
+  DICTIONARY32, STRING, LIST, DECIMAL32, DECIMAL64, DECIMAL128, STRUCT, NUM_TYPE_IDS  // no column of these types exists here
 };
 class data_type {
  public:
@@ -977,5 +978,51 @@ inline std::unique_ptr<column> distinct_indices(table_view const& input, duplica
                                     stream.value(), &out));
   return std::make_unique<column>(out);
 }
+
+// binaryop.hpp (cpp/include/cudf/binaryop.hpp:30-84,158-294): fixed-width columns and scalars; the semantics, undefined values
+// and errors are b2_binary_operation's (include/cudf_b200.h). An unsupported combination is cudf::data_type_error, differing
+// column sizes std::invalid_argument, a type id outside type_id cudf::logic_error.
+enum class binary_operator : int32_t {
+  ADD, SUB, MUL, DIV, TRUE_DIV, FLOOR_DIV, MOD, PMOD, PYMOD, POW, INT_POW, LOG_BASE, ATAN2, SHIFT_LEFT, SHIFT_RIGHT,
+  SHIFT_RIGHT_UNSIGNED, BITWISE_AND, BITWISE_OR, BITWISE_XOR, LOGICAL_AND, LOGICAL_OR, EQUAL, NOT_EQUAL, LESS, GREATER,
+  LESS_EQUAL, GREATER_EQUAL, NULL_EQUALS, NULL_NOT_EQUALS, NULL_MAX, NULL_MIN, GENERIC_BINARY, NULL_LOGICAL_AND,
+  NULL_LOGICAL_OR, INVALID_BINARY
+};
+inline std::unique_ptr<column> binary_operation(scalar const& lhs, column_view const& rhs, binary_operator op, data_type output_type,
+                                                rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_binary_operation_sc(lhs.native(), &rhs.native(), static_cast<int32_t>(op), static_cast<int32_t>(output_type.id()),
+                                       stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> binary_operation(column_view const& lhs, scalar const& rhs, binary_operator op, data_type output_type,
+                                                rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_binary_operation_cs(&lhs.native(), rhs.native(), static_cast<int32_t>(op), static_cast<int32_t>(output_type.id()),
+                                       stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> binary_operation(column_view const& lhs, column_view const& rhs, binary_operator op,
+                                                data_type output_type, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_binary_operation(&lhs.native(), &rhs.native(), static_cast<int32_t>(op), static_cast<int32_t>(output_type.id()),
+                                    stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+namespace binops {
+inline bool is_supported_operation(data_type out, data_type lhs, data_type rhs, binary_operator op)
+{
+  int32_t r = 0;
+  detail::check(b2_binary_is_supported_operation(static_cast<int32_t>(out.id()), static_cast<int32_t>(lhs.id()),
+                                                 static_cast<int32_t>(rhs.id()), static_cast<int32_t>(op), &r));
+  return r != 0;
+}
+}  // namespace binops
 
 }  // namespace cudf

@@ -357,6 +357,51 @@ B2_API b2_status b2_distinct(const b2_table_view* input, const int32_t* keys, in
 B2_API b2_status b2_distinct_indices(const b2_table_view* input, int32_t keep, int32_t nulls_equal, int32_t nans_equal,
                                      b2_stream stream, b2_column** out);
 
+/* ---- binary operations: cpp/include/cudf/binaryop.hpp, cpp/src/binaryop/binaryop.cpp, cpp/src/binaryop/compiled/* -----------
+ * out[i] = op(lhs[i], rhs[i]) over fixed-width columns, or a column and a scalar (a scalar operand is the same value in every
+ * row).  The operator values are cudf::binary_operator's.  Types: INT8..UINT64, FLOAT32, FLOAT64 and BOOL8 in any combination
+ * of lhs, rhs and output; a timestamp or duration operand only against the same type id, for the six comparisons,
+ * NULL_EQUALS / NULL_NOT_EQUALS (output BOOL8) and NULL_MAX / NULL_MIN (output of the operands' type), on the storage integers.
+ *  - Compute type C = std::common_type<out, lhs, rhs> (for a chrono comparison: the operands' storage type).  The value is
+ *    Out(op(C(x), C(y))) with C++ semantics: integers narrower than 32 bits are computed as int and wrap on the cast to Out,
+ *    signed overflow wraps; TRUE_DIV, POW, LOG_BASE, ATAN2 and PYMOD on floats compute in double; FLOOR_DIV rounds toward
+ *    -inf for integers and is floor(x / y) for floats; MOD on floats is fmod; INT_POW is exponentiation by squaring in C and 0
+ *    for a negative exponent; comparisons and logical operators write BOOL8.
+ *  - Validity: the AND of the operands' (a null scalar makes every row null), except for the null-aware operators, whose
+ *    output always has a mask: NULL_EQUALS(null, null) = true, NULL_EQUALS(null, x) = false, NULL_NOT_EQUALS its negation,
+ *    all valid; NULL_MAX / NULL_MIN take the valid operand, null when both are; NULL_LOGICAL_AND(null, false) = false,
+ *    NULL_LOGICAL_OR(null, true) = true, otherwise null when an operand is.  The output has a mask when a row can be null;
+ *    null_count is exact.  An empty column gives an empty column of the output type.
+ *  - Undefined values (as in the reference; no result depends on them): integer division or modulo by zero and INT_MIN / -1
+ *    (DIV, FLOOR_DIV, MOD, PMOD, PYMOD), shifts by a negative amount or at / beyond the width of the promoted left operand,
+ *    float-to-integer conversions of NaN or of values whose integer part the output type cannot hold, integer-only operators
+ *    (INT_POW, shifts, bitwise) whose C is a float because the output is (here computed in std::common_type<lhs, rhs>), and
+ *    values under null bits.
+ *  - Errors: column sizes differ -> INVALID_ARGUMENT; a type id outside cudf::type_id -> LOGIC; GENERIC_BINARY, an operator
+ *    outside the enum, decimal / string / nested types and every other unsupported combination -> DATA_TYPE.
+ *  - The scalar forms read the scalar's validity back (one synchronisation of `stream`), as the reference does; the column
+ *    form does not synchronise. */
+enum {
+  B2_BINOP_ADD = 0, B2_BINOP_SUB = 1, B2_BINOP_MUL = 2, B2_BINOP_DIV = 3, B2_BINOP_TRUE_DIV = 4, B2_BINOP_FLOOR_DIV = 5,
+  B2_BINOP_MOD = 6, B2_BINOP_PMOD = 7, B2_BINOP_PYMOD = 8, B2_BINOP_POW = 9, B2_BINOP_INT_POW = 10, B2_BINOP_LOG_BASE = 11,
+  B2_BINOP_ATAN2 = 12, B2_BINOP_SHIFT_LEFT = 13, B2_BINOP_SHIFT_RIGHT = 14, B2_BINOP_SHIFT_RIGHT_UNSIGNED = 15,
+  B2_BINOP_BITWISE_AND = 16, B2_BINOP_BITWISE_OR = 17, B2_BINOP_BITWISE_XOR = 18, B2_BINOP_LOGICAL_AND = 19,
+  B2_BINOP_LOGICAL_OR = 20, B2_BINOP_EQUAL = 21, B2_BINOP_NOT_EQUAL = 22, B2_BINOP_LESS = 23, B2_BINOP_GREATER = 24,
+  B2_BINOP_LESS_EQUAL = 25, B2_BINOP_GREATER_EQUAL = 26, B2_BINOP_NULL_EQUALS = 27, B2_BINOP_NULL_NOT_EQUALS = 28,
+  B2_BINOP_NULL_MAX = 29, B2_BINOP_NULL_MIN = 30, B2_BINOP_GENERIC_BINARY = 31, B2_BINOP_NULL_LOGICAL_AND = 32,
+  B2_BINOP_NULL_LOGICAL_OR = 33, B2_BINOP_INVALID_BINARY = 34
+};
+B2_API b2_status b2_binary_operation(const b2_column_view* lhs, const b2_column_view* rhs, int32_t op, int32_t out_type,
+                                     b2_stream stream, b2_column** out);
+B2_API b2_status b2_binary_operation_cs(const b2_column_view* lhs, const b2_scalar* rhs, int32_t op, int32_t out_type,
+                                        b2_stream stream, b2_column** out);
+B2_API b2_status b2_binary_operation_sc(const b2_scalar* lhs, const b2_column_view* rhs, int32_t op, int32_t out_type,
+                                        b2_stream stream, b2_column** out);
+/* cudf::binops::is_supported_operation: *result = 1 when the call above accepts (out, lhs, rhs, op); type ids outside
+ * cudf::type_id -> LOGIC. */
+B2_API b2_status b2_binary_is_supported_operation(int32_t out_type, int32_t lhs_type, int32_t rhs_type, int32_t op,
+                                                  int32_t* result);
+
 /* Two-phase form of b2_partition for the fused partition + exchange: the plan holds the bucket id and the
  * stable in-bucket rank of every row; out_counts[b] = rows of bucket b.  b2_partition_scatter then writes one
  * fixed-width column straight to P destination base addresses — local buffers or PEER device memory mapped with

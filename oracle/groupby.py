@@ -58,9 +58,19 @@ def result_dtype(kind, in_dtype):
     return in_dtype
 
 
-def aggregate(key_cols, requests, null_handling=EXCLUDE):
+def takes_sort_path(requests) -> bool:
+    """cpp/src/groupby/groupby.cu:65-69: a request holding an aggregation without a hash implementation sends the whole call
+    down the sort-based path (as do keys declared sorted, which the oracle is not told about)."""
+    return any((k[0] if isinstance(k, tuple) else k) in (MEDIAN, NUNIQUE, NTH_ELEMENT) for _, kinds in requests for k in kinds)
+
+
+def aggregate(key_cols, requests, null_handling=EXCLUDE, sort_path=None):
     """requests: list of ((values, valid), [kinds]).
+    sort_path: M2 / VARIANCE / STD as the sort-based path computes them (two passes) rather than the hash path's one-pass
+    formula; None decides as the reference's dispatch does (takes_sort_path).
     -> (key columns [(values, valid)], results[request][kind] = (values, valid | None))."""
+    if sort_path is None:
+        sort_path = takes_sort_path(requests)
     n = len(key_cols[0][0]) if key_cols else 0
     for (vals, _), _k in requests:
         if len(vals) != n:
@@ -100,13 +110,30 @@ def aggregate(key_cols, requests, null_handling=EXCLUDE):
                         per.append((sq.astype(rdt), (vc > 0) if has_nulls else None))
                         continue
                     cnt = np.maximum(vc, 1).astype(np.float64)
-                    m2v = np.where(vc == 0, 0.0, sq.astype(np.float64) - sm.astype(np.float64) * sm.astype(np.float64) / cnt)
-                    if kind == M2:
-                        per.append((m2v, None))
-                        continue
                     df = vc - ddof
                     ok = (vc != 0) & (df > 0)
-                    var = np.where(ok, m2v / np.where(ok, df, 1), 0.0)
+                    if sort_path:
+                        # two passes in float64 (cpp/src/groupby/sort/group_m2.cu:34-58, group_std.cu:19-52): the group MEAN, then
+                        # (x - mean)^2 per value, divided by (n - ddof) for VARIANCE / STD, summed; STD = sqrt(VARIANCE)
+                        xd = xv.astype(np.float64)
+                        s1 = np.zeros(ng)
+                        np.add.at(s1, xg, xd)
+                        d = xd - (s1 / cnt)[xg]
+                        t = d * d
+                        if kind != M2:
+                            t = np.where(ok[xg], t / np.where(ok, df, 1)[xg], 0.0)
+                        acc = np.zeros(ng)
+                        np.add.at(acc, xg, t)
+                        if kind == M2:
+                            per.append((acc, None))
+                            continue
+                        var = np.where(ok, acc, 0.0)
+                    else:
+                        m2v = np.where(vc == 0, 0.0, sq.astype(np.float64) - sm.astype(np.float64) * sm.astype(np.float64) / cnt)
+                        if kind == M2:
+                            per.append((m2v, None))
+                            continue
+                        var = np.where(ok, m2v / np.where(ok, df, 1), 0.0)
                     out = var if kind == VARIANCE else np.sqrt(np.where(ok, var, 0.0))
                 per.append((out, None if ok.all() else ok))
                 continue
@@ -128,13 +155,17 @@ def aggregate(key_cols, requests, null_handling=EXCLUDE):
                             x = np.where(x == 0, 0.0, x)          # -0 == +0; np.unique treats NaNs as one value
                         out[g] = len(np.unique(x))
                     else:
-                        x = np.sort(gv[gm].astype(np.float64))
+                        # ranked in the value type (stable, -0 == +0, NaN last), then interpolate::linear
+                        # (cpp/src/quantiles/quantiles_util.hpp:23-36,73-89): (1 - f) * a + f * b, each product rounded on its own
+                        x = np.sort(gv[gm], kind="stable").astype(np.float64)
                         if len(x) == 0:
                             ok[g] = False
                         else:
                             pos = (len(x) - 1) * 0.5
                             lo, hi = int(np.floor(pos)), int(np.ceil(pos))
-                            out[g] = x[lo] + (pos - lo) * (x[hi] - x[lo])
+                            f = np.float64(pos - lo)
+                            with np.errstate(invalid="ignore", over="ignore"):
+                                out[g] = (np.float64(1.0) - f) * x[lo] + f * x[hi]
                 per.append((out, None if (kind == NUNIQUE or ok.all()) else ok))
                 continue
             if kind in (ARGMAX, ARGMIN):

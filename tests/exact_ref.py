@@ -183,6 +183,27 @@ def var_std_bounds(k: int, x, ddof: int):
     return var, bv, std, bs
 
 
+def two_pass_bounds(k: int, x, delta: float, ddof: int):
+    """Forward error of the sort path's two-pass M2 / VARIANCE / STD (group_m2.cu, group_std.cu) over finite x, with the group
+    mean computed to within delta and the per-row terms summed along chains of length k.
+
+    sum((x - m)^2) = M2 + n (m - mean)^2 exactly for any m, so the computed mean adds at most n delta^2. Each term is rounded
+    by the difference and the square (and the division by n - ddof for VARIANCE), and the sum of those non-negative terms adds
+    k u relative; (2k + 3) u covers both with room for the second-order terms.
+    -> (M2, its bound, VAR, its bound, STD, its bound); VAR / STD are None when n <= ddof."""
+    n = len(x)
+    m2 = exact_m2(x)
+    shift = n * delta * delta
+    bm = shift + (2 * k + 3) * U64 * (m2 + shift) + U64 * m2
+    if n - ddof <= 0:
+        return m2, bm, None, None, None, None
+    var = m2 / (n - ddof)
+    bv = (shift + (2 * k + 4) * U64 * (m2 + shift)) / (n - ddof) + U64 * var
+    std = math.sqrt(var)
+    bs = max(math.sqrt(var + bv) - std, std - math.sqrt(max(var - bv, 0.0))) + 2 * U64 * std
+    return m2, bm, var, bv, std, bs
+
+
 def check(got, exact, bound, what=""):
     """got within bound of exact; NaN / inf results are compared as values."""
     got, exact = float(got), float(exact)

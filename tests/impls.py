@@ -37,8 +37,8 @@ class OracleImpl:
         """The whole join, however it is partitioned (the partitioned API must reproduce it)."""
         return getattr(ojoin, f"{kind}_join")(l, r, ne)
 
-    def groupby(self, keys, requests, include_nulls=False):
-        k, res = ogb.aggregate(keys, [(c, [KINDS[x] for x in kinds]) for c, kinds in requests], 1 if include_nulls else 0)
+    def groupby(self, keys, requests, include_nulls=False, sort_path=None):
+        k, res = ogb.aggregate(keys, [(c, [KINDS[x] for x in kinds]) for c, kinds in requests], 1 if include_nulls else 0, sort_path)
         return k, res
 
     def groupby_scan(self, keys, requests, include_nulls=False):

@@ -441,7 +441,18 @@ def groupby_results(plc):
 
 
 def _k_path(path, count):
+    """Longest addition chain behind a group's SUM / MEAN (and, on the hash and partitioned paths, the one-pass M2's SUM and
+    SUM_OF_SQUARES): atomics land in any order there; the sort path reduces each group with segmented_reduce, whose MEAN also
+    rounds each value on its way to float64 (+1)."""
     return X.k_hash_group(count) if path != "sort" else X.k_segmented(count) + 1
+
+
+def _two_pass(rows, xv, ddof):
+    """The sort path's two-pass bounds for a group of `rows` rows (nulls included: segmented_reduce walks them all) whose valid
+    values are xv: the MEAN to within mean_bound, the squared deviations summed by segmented_reduce."""
+    k = X.k_segmented(rows)
+    delta = X.mean_bound(k + 1, X.U64, X.abs_sum(xv), X.exact_sum(xv), len(xv), X.U64)
+    return X.two_pass_bounds(k, xv, delta, ddof)
 
 
 @pytest.mark.parametrize("path", ["hash", "sort", "partitioned", "partitioned-spill"])
@@ -484,12 +495,19 @@ def test_groupby_bounds(groupby_results, path):
                 finite = np.isfinite(xv).all()
                 if not finite:
                     assert math.isnan(r["m2"][0]), what
+                elif path == "sort":  # two passes: never negative
+                    m2, bm, var, bv, std, bs = _two_pass(int((keys == key).sum()), xv.astype(np.float64), 1)
+                    assert r["m2"][0] >= 0, what
+                    X.check(r["m2"][0], m2, bm, "m2 " + what)
                 else:
                     X.check(r["m2"][0], X.exact_m2(xv), X.m2_bound(k, xv), "m2 " + what)
                 assert r["var"][1] == (len(xv) > 1) and r["std"][1] == (len(xv) > 1), what
                 if len(xv) > 1:
                     if not finite:
                         assert math.isnan(r["var"][0]) and math.isnan(r["std"][0]), what
+                    elif path == "sort":
+                        X.check(r["var"][0], var, bv, "var " + what)
+                        X.check(r["std"][0], std, bs, "std " + what)
                     else:
                         var, bv, std, bs = X.var_std_bounds(k, xv, 1)
                         X.check(r["var"][0], var, bv, "var " + what)
@@ -502,17 +520,23 @@ def test_groupby_bounds(groupby_results, path):
 
 
 def test_groupby_large_mean_small_spread_matches_the_one_pass_formula(groupby_results):
-    """M2 = sumsq - sum^2 / n loses most of its digits here; each path stays within that formula's bound and no tighter
-    claim is made (the bound is many times the two-pass formula's error)."""
+    """The hash path's M2 = sumsq - sum^2 / n (the reference's hash formula) loses most of its digits here: it stays within
+    that formula's bound and no tighter claim is made. The sort path takes two passes, as the reference's sort path does, and
+    is held to that algorithm's bound, which is many times tighter."""
     for path in ("hash", "sort"):
         case, kinds, (gk, res) = groupby_results[(path, "large-mean")]
         _, keys, x, _, _ = case
         m2 = res[kinds.index("m2")][0]
         for gi, key in enumerate(gk):
             xv = x[keys == key]
-            bound = X.m2_bound(_k_path(path, len(xv)), xv)
-            assert bound > 1e-3 * X.exact_m2(xv)  # the formula cannot promise better than ~0.1 % here
-            X.check(m2[gi], X.exact_m2(xv), bound, f"{path} key={key}")
+            one_pass = X.m2_bound(_k_path(path, len(xv)), xv)
+            assert one_pass > 1e-3 * X.exact_m2(xv)  # the one-pass formula cannot promise better than ~0.1 % here
+            if path == "hash":
+                X.check(m2[gi], X.exact_m2(xv), one_pass, f"{path} key={key}")
+            else:
+                exact, bound = _two_pass(len(xv), xv, 0)[:2]
+                assert bound < 1e-9 * exact
+                X.check(m2[gi], exact, bound, f"{path} key={key}")
 
 
 def test_groupby_min_max_arg_agree_across_paths(groupby_results):

@@ -136,3 +136,24 @@ def test_mix64_shuffle_bucket_pinned():
         assert b.min() >= 0 and b.max() < P
         assert np.abs(np.bincount(b, minlength=P) / len(k) - 1 / P).max() < 0.01
         assert b[0] == (((fmix(((int(k[0]) & M) ^ (1 << 63)) + 0x9E3779B97F4A7C15 & M) >> 32) * P) >> 32)
+
+
+def test_groupby_median_interpolation():
+    """MEDIAN is interpolate::linear, (1 - f) * a + f * b (cpp/src/quantiles/quantiles_util.hpp:23-36), not a + f * (b - a):
+    the two differ on infinities, on opposite values near DBL_MAX and in the last bit of ordinary pairs."""
+    from oracle import groupby as ogb
+
+    inf, nan, big = np.inf, np.nan, 1.5e308
+    groups = [[-inf, 5.0], [inf, inf], [-inf, -inf], [-big, big], [1.049001171530397, 6.40422650443282], [inf], [1.0, nan],
+              [3.0, nan, 1.0], [2.0, -0.0, 0.0]]
+    exp = [-inf, inf, -inf, 0.0, 3.726613837981609, nan, nan, 3.0, 0.0]
+    keys = np.repeat(np.arange(len(groups)), [len(g) for g in groups])
+    vals = np.concatenate([np.array(g) for g in groups])
+    _, res = ogb.aggregate([(keys, None)], [((vals, None), [ogb.MEDIAN])])
+    got, ok = res[0][0]
+    assert ok is None
+    assert np.array_equal(got, np.array(exp), equal_nan=True), got
+    # integers convert to double before interpolating, without a signed detour: UINT64 above 2^63 stays positive
+    u = np.array([2**63 + 2048, 2**63 + 2048, 2**64 - 1], np.uint64)
+    _, res = ogb.aggregate([(np.zeros(3, np.int32), None)], [((u, None), [ogb.MEDIAN])])
+    assert res[0][0][0].tolist() == [float(2**63 + 2048)]

@@ -1264,6 +1264,16 @@ __global__ void gb_squares_kernel(const void* __restrict__ src, int32_t st, int6
     if (i2) i2[i] = (long long)((unsigned long long)w * (unsigned long long)w);
   }
 }
+// MEAN of an integral column on the sort path, as the reference's (aggregate.cpp:275-298: a DIV of the SUM and COUNT_VALID results,
+// in double) and the hash path's finalize_kernel: the group's wrapped INT64 SUM over its valid count. In place: sum and out may alias.
+__global__ void gb_int_mean_kernel(const long long* sum, const int32_t* __restrict__ cnt, int32_t G, double* out)
+{
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= G) return;
+  const int32_t c = cnt[g];
+  const long long s = sum[g];
+  out[g] = c > 0 ? (double)s / (double)c : 0.0;
+}
 // The sort path's M2 / VARIANCE / STD take two passes, as the reference's sort path does (cpp/src/groupby/sort/group_m2.cu:34-58,
 // group_std.cu:19-52, aggregate.cpp:303-353): the group MEAN first, then per valid row (x - mean)^2, divided by (n - ddof) for
 // VARIANCE / STD, summed per group. Null rows and rows of a group with n <= ddof contribute 0.
@@ -1493,6 +1503,18 @@ void groupby_aggregate_sorted(const b2_groupby& gb, const std::vector<request_vi
       }
       return *vs2;
     };
+    // MEAN (alone, and the first pass of M2 / VARIANCE / STD): for integral values the INT64 SUM over the valid count, so that a
+    // sum above 2^53 or one that wraps gives the reference's result; float values are converted to double and summed in double
+    auto group_mean = [&](const b2_column_view& xv) -> column_ptr {
+      if (!is_integral_id(st)) return segmented_reduce(xv, off, G + 1, B2_AGG_MEAN, B2_FLOAT64, B2_NULL_EXCLUDE, nullptr, stream);
+      b2_column_view sv = vsv;
+      sv.type_id = st;
+      auto col = segmented_reduce(sv, off, G + 1, B2_AGG_SUM, B2_INT64, B2_NULL_EXCLUDE, nullptr, stream);
+      const int32_t* vc = valid_counts();
+      B2_LAUNCH(gb_int_mean_kernel, ggrid, 256, 0, stream, col->data.as<long long>(), vc, G, col->data.as<double>());
+      col->type_id = B2_FLOAT64;
+      return col;
+    };
     for (int32_t raw : r.kinds) {
       const int32_t kind = base_kind(raw);
       const int32_t rt = sorted_result_type(kind, v.type_id);
@@ -1506,7 +1528,8 @@ void groupby_aggregate_sorted(const b2_groupby& gb, const std::vector<request_vi
       } else if (kind == B2_AGG_SUM || kind == B2_AGG_PRODUCT || kind == B2_AGG_MIN || kind == B2_AGG_MAX || kind == B2_AGG_MEAN) {
         b2_column_view sv = vsv;
         sv.type_id = (kind == B2_AGG_MIN || kind == B2_AGG_MAX) ? vsv.type_id : st;  // chrono sums go through their integer storage
-        col = segmented_reduce(sv, off, G + 1, kind, (kind == B2_AGG_MIN || kind == B2_AGG_MAX) ? vsv.type_id : rt, B2_NULL_EXCLUDE, nullptr, stream);
+        if (kind == B2_AGG_MEAN) col = group_mean(sv);
+        else col = segmented_reduce(sv, off, G + 1, kind, (kind == B2_AGG_MIN || kind == B2_AGG_MAX) ? vsv.type_id : rt, B2_NULL_EXCLUDE, nullptr, stream);
         col->type_id = rt;
         if (!nullable) { col->pending.reset(); col->mask.reset(); col->null_count = 0; }  // a mask only when the input has nulls (output_utils.cu:67-86)
       } else if (needs_sumsq(kind)) {
@@ -1520,7 +1543,7 @@ void groupby_aggregate_sorted(const b2_groupby& gb, const std::vector<request_vi
         } else {
           // two passes (gb_dev2_kernel): the group MEAN, then the sum of the squared deviations from it
           b2_column_view xv{B2_FLOAT64, (int32_t)n, x.ptr, nullable ? vsv.null_mask : nullptr, nullable ? vsv.null_count : 0, 0};
-          auto mean = segmented_reduce(xv, off, G + 1, B2_AGG_MEAN, B2_FLOAT64, B2_NULL_EXCLUDE, nullptr, stream);
+          auto mean = group_mean(xv);
           const bool var_std = kind != B2_AGG_M2;
           const int32_t ddof = kind_ddof(raw);
           const int32_t* vc = valid_counts();  // (evaluated here: launch arguments must not launch kernels themselves)

@@ -210,21 +210,33 @@ void dispatch_reduce_op(int op, const b2_column_view& col, reduce_tail& t, cudaS
   }
 }
 
-// widen: false -> accumulate in the element type itself (output type == input type)
+// unsigned input: accumulate in uint64 when the output is the input type (MIN / MAX need its order), else in int64 as the
+// reference does (simple.cuh:407-419): the bits are the same, but a result with bit 63 set converts to a negative float
+template <typename T>
+void dispatch_reduce_unsigned(bool widen, int op, const b2_column_view& col, reduce_tail& t, cudaStream_t stream)
+{
+  if (widen) {
+    if (op == OP_SUM) launch_reduce<T, int64_t, OP_SUM>(col, t, stream);
+    else launch_reduce<T, int64_t, OP_PRODUCT>(col, t, stream);  // MIN / MAX: output type == input type
+  } else {
+    dispatch_reduce_op<T, uint64_t>(op, col, t, stream);
+  }
+}
+
+// widen: true -> the output type differs from the input type: integers accumulate in int64, floats in double
 void dispatch_reduce(int32_t in_type, bool widen, bool to_float32_acc, int op, const b2_column_view& col, reduce_tail& t,
                      cudaStream_t stream)
 {
-  (void)widen;
   switch (in_type) {
     // integer accumulation in 64 bits truncates to the same bits as narrow wrap-around arithmetic
     case B2_INT8: dispatch_reduce_op<int8_t, int64_t>(op, col, t, stream); break;
     case B2_INT16: dispatch_reduce_op<int16_t, int64_t>(op, col, t, stream); break;
     case B2_INT32: dispatch_reduce_op<int32_t, int64_t>(op, col, t, stream); break;
     case B2_INT64: dispatch_reduce_op<int64_t, int64_t>(op, col, t, stream); break;
-    case B2_UINT8: case B2_BOOL8: dispatch_reduce_op<uint8_t, uint64_t>(op, col, t, stream); break;
-    case B2_UINT16: dispatch_reduce_op<uint16_t, uint64_t>(op, col, t, stream); break;
-    case B2_UINT32: dispatch_reduce_op<uint32_t, uint64_t>(op, col, t, stream); break;
-    case B2_UINT64: dispatch_reduce_op<uint64_t, uint64_t>(op, col, t, stream); break;
+    case B2_UINT8: case B2_BOOL8: dispatch_reduce_unsigned<uint8_t>(widen, op, col, t, stream); break;
+    case B2_UINT16: dispatch_reduce_unsigned<uint16_t>(widen, op, col, t, stream); break;
+    case B2_UINT32: dispatch_reduce_unsigned<uint32_t>(widen, op, col, t, stream); break;
+    case B2_UINT64: dispatch_reduce_unsigned<uint64_t>(widen, op, col, t, stream); break;
     case B2_FLOAT32:
       if (to_float32_acc) dispatch_reduce_op<float, float>(op, col, t, stream);
       else dispatch_reduce_op<float, double>(op, col, t, stream);
@@ -661,12 +673,15 @@ column_ptr scan(const b2_column_view& col, int32_t kind, int32_t scan_type, int3
   b2_column_view c2 = col;
   c2.null_mask = scan_mask;
   (void)scan_mask_offset;
+  // a running SUM of BOOL8 is true from the first true row on (the reference adds bools as ints and stores bool): MAX of the
+  // 0 / 1 bytes, which a uint8 + would wrap back to 0 after 256 true rows
+  const int sop = sid == B2_BOOL8 && op == OP_SUM ? OP_MAX : op;
   switch (sid) {
     case B2_INT8: dispatch_scan_op<int8_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_INT16: dispatch_scan_op<int16_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_INT32: dispatch_scan_op<int32_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_INT64: dispatch_scan_op<int64_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
-    case B2_UINT8: case B2_BOOL8: dispatch_scan_op<uint8_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
+    case B2_UINT8: case B2_BOOL8: dispatch_scan_op<uint8_t>(sop, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_UINT16: dispatch_scan_op<uint16_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_UINT32: dispatch_scan_op<uint32_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
     case B2_UINT64: dispatch_scan_op<uint64_t>(op, c2, scan_mask, exclusive, out->data.ptr, stream); break;
@@ -825,15 +840,17 @@ column_ptr segmented_reduce(const b2_column_view& col, const int32_t* offsets, i
       default: B2_FAIL(B2_ERR_DATA_TYPE, "unsupported type for segmented_reduce");
     }
   } else {
+    // unsigned inputs: uint64 when the output is the input type (MIN / MAX order), else int64 like the signed ones
+    // (segmented/simple.cuh reduce_numeric): a sum with bit 63 set then converts to a negative float, as in the reference
     switch (sid) {
       case B2_INT8: SEG(int8_t, int64_t); break;
       case B2_INT16: SEG(int16_t, int64_t); break;
       case B2_INT32: SEG(int32_t, int64_t); break;
       case B2_INT64: SEG(int64_t, int64_t); break;
-      case B2_UINT8: case B2_BOOL8: SEG(uint8_t, uint64_t); break;
-      case B2_UINT16: SEG(uint16_t, uint64_t); break;
-      case B2_UINT32: SEG(uint32_t, uint64_t); break;
-      case B2_UINT64: SEG(uint64_t, uint64_t); break;
+      case B2_UINT8: case B2_BOOL8: if (same) SEG(uint8_t, uint64_t); else SEG(uint8_t, int64_t); break;
+      case B2_UINT16: if (same) SEG(uint16_t, uint64_t); else SEG(uint16_t, int64_t); break;
+      case B2_UINT32: if (same) SEG(uint32_t, uint64_t); else SEG(uint32_t, int64_t); break;
+      case B2_UINT64: if (same) SEG(uint64_t, uint64_t); else SEG(uint64_t, int64_t); break;
       case B2_FLOAT32: if (same) SEG(float, float); else SEG(float, double); break;
       case B2_FLOAT64: SEG(double, double); break;
       default: B2_FAIL(B2_ERR_DATA_TYPE, "unsupported type for segmented_reduce");

@@ -115,9 +115,10 @@ def aggregate(key_cols, requests, null_handling=EXCLUDE, sort_path=None):
                     if sort_path:
                         # two passes in float64 (cpp/src/groupby/sort/group_m2.cu:34-58, group_std.cu:19-52): the group MEAN, then
                         # (x - mean)^2 per value, divided by (n - ddof) for VARIANCE / STD, summed; STD = sqrt(VARIANCE)
+                        # the MEAN is the sort path's: SUM / COUNT_VALID (aggregate.cpp:275-298), with an integral SUM in (wrapping)
+                        # int64, so a UINT64 value at or above 2^63 or a sum past 2^63 shifts the mean as in the reference
                         xd = xv.astype(np.float64)
-                        s1 = np.zeros(ng)
-                        np.add.at(s1, xg, xd)
+                        s1 = sm.astype(np.float64)
                         d = xd - (s1 / cnt)[xg]
                         t = d * d
                         if kind != M2:

@@ -407,7 +407,13 @@ struct pass_args {
   const void* val_in;       // CARRY kernels: the caller's payload column (first pass source); last member on purpose
   // RANGE kernels (sharded sort: the range partition IS the exchange): digit = number of splitters <= key; the rows of digit d
   // are written to range_key_dst[d] / range_val_dst[d] (local or PEER memory) at their rank inside this GPU's digit-d run
-  const void* range_splitters;       // device array of (range_parts - 1) twiddled keys, ascending
+  // EST kernels share the slot (the parameter block keeps its size): tile table of the estimated-base second pass (run_est_range):
+  // tile t reads rows [x, x + (y & 0x7fffffff)) of its source (one window of the first pass), y >> 31 marks the last tile, y == 0
+  // lies past the last tile
+  union {
+    const void* range_splitters;     // device array of (range_parts - 1) twiddled keys, ascending
+    const uint2* est_tiles;
+  };
   void* const* range_key_dst;        // device array of range_parts pointers
   void* const* range_val_dst;        // same for the carried payload (CARRY) or null
   int32_t range_parts;
@@ -599,7 +605,10 @@ using tile_384x16      = tile_shape<384, 16, 2>;        // 8-byte keys: row ids,
 using tile_512x16      = tile_shape<512, 16, 1>;        // 1-, 2- and 4-byte keys
 using tile_512x20_bulk = tile_shape<512, 20, 1, true>;  // 8-byte keys carrying 8-byte payloads
 
-template <typename UK, typename Shape, typename VT, bool CARRY, bool MIX, bool RANGE>
+// EST (64-bit raw keys, range sort with estimated bases): digit d owns rows [d * est_cap, (d + 1) * est_cap) of the output (overflow
+// check as MIX), the last tile publishes every digit's end, and the first pass ORs (key ^ first key) into ctl->vary; with est_tiles
+// the tiles come from that table (the windows of the first pass) instead of one contiguous portion.
+template <typename UK, typename Shape, typename VT, bool CARRY, bool MIX, bool RANGE, bool EST = false>
 __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) onesweep_kernel(pass_args a)
 {
   constexpr int THREADS = Shape::threads;
@@ -633,7 +642,19 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
   const int warp = tid >> 5;
   const bool ranker = warp < NWARPS;
 
-  if (tid == 0) s_misc[0] = atomicAdd(a.tile_counter, 1u);
+  if (tid == 0) {
+    const uint32_t t = atomicAdd(a.tile_counter, 1u);
+    s_misc[0] = t;
+    if constexpr (EST) {
+      s_misc[10] = 0;  // the tile's vary word
+      s_misc[11] = 0;
+      if (a.est_tiles != nullptr) {
+        const uint2 e = a.est_tiles[t];
+        s_misc[9]  = e.x;
+        s_misc[14] = e.y;
+      }
+    }
+  }
   if constexpr (BULK && !EMU_BUILD) {
     if (tid == 0) mbar_init_one((uint32_t)__cvta_generic_to_shared(s_misc + 12));  // 8-byte aligned slot behind the scan scratch (s_misc[1..8])
   }
@@ -653,8 +674,17 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
   }
   __syncthreads();
   const uint32_t tile = s_misc[0];
-  const uint32_t tile_base = tile * (uint32_t)TILE;  // within portion
-  const uint32_t tile_n = min((uint32_t)TILE, a.portion_n - tile_base);
+  uint32_t tile_base = tile * (uint32_t)TILE;  // within portion (EST table: first source row of the tile)
+  uint32_t tile_n = min((uint32_t)TILE, a.portion_n - tile_base);
+  uint32_t nlim = a.portion_n;                 // source rows below nlim exist
+  if constexpr (EST) {
+    if (a.est_tiles != nullptr) {
+      if (s_misc[14] == 0) return;  // past the last tile: the whole CTA leaves before the named barriers
+      tile_base = s_misc[9];
+      tile_n    = s_misc[14] & 0x7fffffffu;
+      nlim      = tile_base + tile_n;
+    }
+  }
   const bool full = tile_n == (uint32_t)TILE;
   const uint32_t pad = (uint32_t)TILE - tile_n;      // padding items sit at the end of digit 255
   const int shift = a.pass * RADIX_BITS;
@@ -718,8 +748,12 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     }
     const uint32_t* gb = &a.ctl->base[a.portion_parity][a.pass][d0];
     bool wants_end = a.has_next_portion != 0;
-    if constexpr (MIX) wants_end = wants_end || a.est_cap != 0u;
-    const bool last_of_portion = wants_end && tile_base + tile_n == a.portion_n;
+    if constexpr (MIX || EST) wants_end = wants_end || a.est_cap != 0u;
+    bool last_tile = tile_base + tile_n == a.portion_n;
+    if constexpr (EST) {
+      if (a.est_tiles != nullptr) last_tile = (s_misc[14] >> 31) != 0u;
+    }
+    const bool last_of_portion = wants_end && last_tile;
 #pragma unroll
     for (int j = 0; j < DPL; ++j) {
       const uint32_t g = gb[j];
@@ -760,7 +794,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 #pragma unroll
       for (int i = 0; i < IPT; ++i) {
         uint32_t e = wbase + i * 32;
-        key[i] = e < a.portion_n ? ld_stream(src + e) : UK(0);
+        key[i] = e < nlim ? ld_stream(src + e) : UK(0);
       }
     }
     if (pl.key_src == 0) {
@@ -774,7 +808,22 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       // padding items take the maximum key so that they rank last in the tile
 #pragma unroll
       for (int i = 0; i < IPT; ++i)
-        if (wbase + i * 32 >= a.portion_n) key[i] = ~UK(0);
+        if (wbase + i * 32 >= nlim) key[i] = ~UK(0);
+    }
+    if constexpr (EST) {
+      if (pl.key_src == 0) {  // first pass: OR of (key ^ first key of the column), the range sort's bucket bits need it exact
+        const UK k0 = twiddle_rt<UK>(static_cast<const UK*>(a.key_bufs[0])[0], a.kind, desc);
+        uint64_t v = 0;
+#pragma unroll
+        for (int i = 0; i < IPT; ++i)
+          if (wbase + i * 32 < nlim) v |= (uint64_t)(key[i] ^ k0);
+        const uint32_t lo = __reduce_or_sync(0xffffffffu, (uint32_t)v);
+        const uint32_t hi = __reduce_or_sync(0xffffffffu, (uint32_t)(v >> 32));
+        if (lane == 0 && (lo | hi)) {
+          atomicOr(&s_misc[10], lo);
+          atomicOr(&s_misc[11], hi);
+        }
+      }
     }
   }
 
@@ -796,7 +845,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
   unsigned dg[RANGE ? IPT : 1];
   if constexpr (RANGE) {
 #pragma unroll
-    for (int i = 0; i < IPT; ++i) dg[i] = (wbase + i * 32 >= a.portion_n) ? (unsigned)(RADIX - 1) : digit_of(key[i]);  // padding ranks last (digit 255)
+    for (int i = 0; i < IPT; ++i) dg[i] = (wbase + i * 32 >= nlim) ? (unsigned)(RADIX - 1) : digit_of(key[i]);  // padding ranks last (digit 255)
   }
   auto digit_at = [&](int i) -> unsigned {
     if constexpr (RANGE) return dg[i];
@@ -806,6 +855,12 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
   uint32_t* my_hist = s_whist + warp * RADIX;
   const int distinct = warp_digit_counts<IPT>(digit_at, IPT, lane, my_hist);
   ranker_barrier(THREADS);  // (S1)
+  if constexpr (EST) {
+    if (tid == 0 && pl.key_src == 0) {  // one global atomic per CTA
+      const unsigned long long v = ((unsigned long long)s_misc[11] << 32) | s_misc[10];
+      if (v) atomicOr(&a.ctl->vary, v);
+    }
+  }
 
   // ---- per digit: warp counts -> warp offsets; publish the aggregate ---------------------------
   uint32_t tstart = 0, count = 0;
@@ -858,7 +913,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 #pragma unroll
         for (int i = 0; i < IPT; ++i) {
           const uint32_t e = wbase + i * 32;
-          idx[i] = e < a.portion_n ? ld_stream(vsrc + e) : VT(0);
+          idx[i] = e < nlim ? ld_stream(vsrc + e) : VT(0);
         }
       } else {
 #pragma unroll
@@ -873,7 +928,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 #pragma unroll
         for (int i = 0; i < IPT; ++i) {
           uint32_t e = wbase + i * 32;
-          idx[i] = e < a.portion_n ? ld_stream(isrc + e) : VT(0);
+          idx[i] = e < nlim ? ld_stream(isrc + e) : VT(0);
         }
       }
     }
@@ -892,7 +947,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     if constexpr (RANGE) d = s_dig[q];
     else d = (unsigned)(k >> shift) & 255u;
     dst[j] = s_off[d] + q;
-    if constexpr (MIX) {
+    if constexpr (MIX || EST) {
       if (a.est_cap != 0u && dst[j] >= (d + 1u) * a.est_cap) {  // digit d's reserved range is full: the caller falls back to exact bases
         if (q < tile_n) a.ctl->overflow = 1u;
         dst[j] = 0xFFFFFFFFu;
@@ -901,7 +956,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     if constexpr (RANGE) {
       dstd[j] = (uint8_t)d;
       if (q < tile_n) static_cast<UK*>(s_kdst[d])[dst[j]] = untwiddle_rt<UK>(k, a.kind, desc);  // the receiver sorts raw column values
-    } else if (write_keys && q < tile_n && (!MIX || dst[j] != 0xFFFFFFFFu)) {
+    } else if (write_keys && q < tile_n && (!(MIX || EST) || dst[j] != 0xFFFFFFFFu)) {
       if (!a.pairs && pl.last && !pl.hybrid) k = untwiddle_rt<UK>(k, a.kind, desc);
       kdst[dst[j]] = k;
     }
@@ -918,7 +973,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       if constexpr (RANGE) {
         if (q < tile_n) static_cast<VT*>(s_vdst[dstd[j]])[dst[j]] = s_vals[q];
       } else {
-        if (q < tile_n && (!MIX || dst[j] != 0xFFFFFFFFu)) idst[dst[j]] = s_vals[q];
+        if (q < tile_n && (!(MIX || EST) || dst[j] != 0xFFFFFFFFu)) idst[dst[j]] = s_vals[q];
       }
     }
   }
@@ -1140,7 +1195,40 @@ __device__ __forceinline__ range_window range_window_load(T* sdst, const T* __re
   return {bulk ? off : 0, bulk};
 }
 
-template <typename VT>
+// Estimated-base range tier (run_est_range): the second pass left output window d7 (rows [d7 * cap, d7 * cap + cnt7[d7]) of its
+// buffers, cnt7 clamped to cap) ordered by digit 6, so range (d7, d6) is contiguous inside it. Block d7, thread d6: est[i] = source
+// start, est[R + i] = rows and est[2R + i] = dense destination (sum_{e < d7} cnt7[e] + offset inside the window) of range i = d7 * 256
+// + d6, R = 65 536. Every range stays inside its window and every destination inside the n output rows, also after an overflow.
+__global__ void __launch_bounds__(RADIX) range_est_bounds_kernel(pass_args a, uint32_t cap, uint32_t* __restrict__ est)
+{
+  __shared__ uint32_t s_lb[RADIX + 1];
+  __shared__ uint32_t s_wsum[RADIX / 32];
+  constexpr int R = RADIX * RADIX;
+  const int d7 = blockIdx.x, d6 = threadIdx.x;
+  const uint64_t* __restrict__ keys = static_cast<const uint64_t*>(a.ctl->fix_key_buf == 1 ? a.key_bufs[1] : a.key_bufs[2]);
+  auto count = [&](int e) { return min(a.ctl->base[1][7][e] - (uint32_t)e * cap, cap); };
+  const uint32_t before = warp_sum(d6 < d7 ? count(d6) : 0u);
+  if ((d6 & 31) == 0) s_wsum[d6 >> 5] = before;
+  const uint32_t w0 = (uint32_t)d7 * cap, wn = count(d7);
+  uint32_t lo = 0, hi = wn;  // first row of the window whose digit 6 is >= d6
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if ((int)((keys[w0 + mid] >> 48) & 255u) < d6) lo = mid + 1;
+    else hi = mid;
+  }
+  s_lb[d6] = lo;
+  if (d6 == 0) s_lb[RADIX] = wn;
+  __syncthreads();
+  uint32_t dense = 0;
+  for (int w = 0; w < RADIX / 32; ++w) dense += s_wsum[w];
+  const uint32_t end = s_lb[d6 + 1];
+  const int i = d7 * RADIX + d6;
+  est[i]         = w0 + lo;
+  est[R + i]     = end > lo ? end - lo : 0u;  // unordered keys (only after an overflow): an empty range
+  est[2 * R + i] = dense + lo;
+}
+
+template <typename VT, bool EST = false>
 __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
 {
   using UK = uint64_t;
@@ -1153,7 +1241,14 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t s = bounds[blockIdx.x];
-  const int m = (int)(bounds[blockIdx.x + 1] - s);
+  int m;
+  int64_t o = s;  // first output row
+  if constexpr (EST) {  // range_est_bounds_kernel's table: source start, rows, dense destination
+    m = (int)bounds[gridDim.x + blockIdx.x];
+    o = bounds[2 * gridDim.x + blockIdx.x];
+  } else {
+    m = (int)(bounds[blockIdx.x + 1] - s);
+  }
   if (m == 0) return;
   if (m > RANGE_CAP) {
     if (tid == 0) atomicOr(&a.ctl->overflow, 1u);
@@ -1161,8 +1256,8 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   }
   const UK* __restrict__ keys = static_cast<const UK*>(a.ctl->fix_key_buf == 1 ? a.key_bufs[1] : a.key_bufs[2]) + s;
   const VT* __restrict__ vin  = reinterpret_cast<const VT*>(a.ctl->fix_idx_buf == 1 ? a.idx_bufs[1] : a.idx_bufs[2]) + s;
-  VT* __restrict__ vout = reinterpret_cast<VT*>(a.idx_bufs[0]) + s;
-  UK* __restrict__ kout = static_cast<UK*>(const_cast<void*>(a.key_bufs[1])) + s;
+  VT* __restrict__ vout = reinterpret_cast<VT*>(a.idx_bufs[0]) + o;
+  UK* __restrict__ kout = static_cast<UK*>(const_cast<void*>(a.key_bufs[1])) + o;
 
   // bucket = the nb bits below the highest bit under the range id that varies over the input (bits between it and the range id
   // are the same in every key); nb ~ log2 m, at most RANGE_BUCKET_BITS. Counter of bucket b: slot (b mod per) * RANGE_THREADS +
@@ -1419,7 +1514,9 @@ int64_t portion_rows(int tile)
 // zero_head() clears (control block, `hist_bytes` of digit histograms, one tile counter per (pass, portion), `tail_bytes` for
 // the caller) and behind it the look-back rows of every (pass, portion), which run() zeroes right before that portion's launch,
 // so that passes the plan skips cost nothing (1e9 rows: 163 MB per executed pass instead of 1.3 GB per sort).
-template <typename UK, typename Shape, typename VT, bool CARRY, bool MIX, bool RANGE = false>
+// extra_tiles: look-back rows for that many tiles more per (pass, portion) (the estimated-base second pass has up to 256 partial
+// tiles in the middle of its sequence).
+template <typename UK, typename Shape, typename VT, bool CARRY, bool MIX, bool RANGE = false, bool EST = false>
 struct onesweep_passes {
   static constexpr int TILE = Shape::tile;
   // every instantiation declares the RANGE arrays behind s_misc, only RANGE launches allocate them
@@ -1431,15 +1528,16 @@ struct onesweep_passes {
   const size_t hist_bytes, cnt_bytes, head_bytes, status_per;
   dbuf work;
 
-  onesweep_passes(int64_t rows, int passes, size_t hist, size_t tail_bytes, cudaStream_t stream)
+  onesweep_passes(int64_t rows, int passes, size_t hist, size_t tail_bytes, cudaStream_t stream, int extra_tiles = 0)
     : n(rows), plim(portion_rows(TILE)), nportions((n + plim - 1) / plim), hist_bytes(hist),
       cnt_bytes((sizeof(uint32_t) * passes * nportions + 255) / 256 * 256), head_bytes(CTL_BYTES + hist_bytes + cnt_bytes + tail_bytes),
-      status_per(sizeof(uint32_t) * RADIX * (size_t)((std::min(n, plim) + TILE - 1) / TILE)),
+      status_per(sizeof(uint32_t) * RADIX * (size_t)((std::min(n, plim) + TILE - 1) / TILE + extra_tiles)),
       work(head_bytes + status_per * passes * nportions, stream)
   {
     static std::atomic<uint64_t> attr_done{0};  // per device: the opt-in to > 48 KB of dynamic shared memory is a per-context setting
     once_per_device(attr_done, [] {
-      B2_CUDA_TRY(cudaFuncSetAttribute(onesweep_kernel<UK, Shape, VT, CARRY, MIX, RANGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM));
+      B2_CUDA_TRY(cudaFuncSetAttribute(onesweep_kernel<UK, Shape, VT, CARRY, MIX, RANGE, EST>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)SMEM));
     });
   }
   sort_ctl* ctl() const { return work.as<sort_ctl>(); }
@@ -1448,12 +1546,12 @@ struct onesweep_passes {
   void zero_head(cudaStream_t stream) const { B2_CUDA_TRY(cudaMemsetAsync(work.ptr, 0, head_bytes, stream)); }
 
   // pass number `slot` of this call, portion by portion (a.pass is the digit it sorts by)
-  void run(pass_args& a, int slot, const char* scope, cudaStream_t stream) const
+  void run(pass_args& a, int slot, const char* scope, cudaStream_t stream, int extra_tiles = 0) const
   {
     for (int64_t q = 0; q < nportions; ++q) {
       const int64_t start = q * plim;
       const int64_t pn = std::min(plim, n - start);
-      const int64_t ntiles = (pn + TILE - 1) / TILE;
+      const int64_t ntiles = (pn + TILE - 1) / TILE + extra_tiles;
       a.portion_start = start;
       a.portion_n = (uint32_t)pn;
       a.portion_parity = (int)(q & 1);
@@ -1462,7 +1560,7 @@ struct onesweep_passes {
       a.tile_counter = reinterpret_cast<uint32_t*>(work.as<char>() + CTL_BYTES + hist_bytes) + slot * nportions + q;
       B2_CUDA_TRY(cudaMemsetAsync(a.status, 0, sizeof(uint32_t) * RADIX * (size_t)ntiles, stream));
       prof_scope ps(scope, stream);
-      B2_LAUNCH((onesweep_kernel<UK, Shape, VT, CARRY, MIX, RANGE>), (unsigned)ntiles, Shape::threads + 32 * LBW, SMEM, stream, a);
+      B2_LAUNCH((onesweep_kernel<UK, Shape, VT, CARRY, MIX, RANGE, EST>), (unsigned)ntiles, Shape::threads + 32 * LBW, SMEM, stream, a);
     }
   }
 };
@@ -1492,6 +1590,123 @@ int64_t hybrid_min_rows()
   return v;
 }
 
+// ---- range tier with estimated bases (no histogram) ---------------------------------------------------------------------------
+// Buffers: keys 0 raw -> 1 (first window buffer) -> 2 (second), payload implicit / carried -> 2 -> 1; the range sort reads key 2 /
+// payload 1 and writes payload 0 (pairs) or key 1, which the host then points at the keys-only output.
+__global__ void range_est_plan_kernel(sort_ctl* ctl, uint32_t cap)
+{
+  const int d = threadIdx.x;  // 256 threads
+  ctl->base[0][6][d] = (uint32_t)d * cap;
+  ctl->base[0][7][d] = (uint32_t)d * cap;
+  if (d < 8) {
+    pass_plan pl{};
+    pl.trivial = d < 6;
+    if (d >= 6) {
+      pl.key_src = d == 6 ? 0 : 1;
+      pl.key_dst = d == 6 ? 1 : 2;
+      pl.idx_src = d == 6 ? -1 : 2;
+      pl.idx_dst = d == 6 ? 2 : 1;
+      pl.last    = d == 7;
+      pl.hybrid  = 1;
+    }
+    ctl->plan[d] = pl;
+  }
+  if (d == 0) {
+    ctl->any_pass    = 2;
+    ctl->hybrid      = 1;
+    ctl->range       = 1;
+    ctl->range_shift = 48;
+    ctl->range_bits  = 16;
+    ctl->fix_shift   = 48;
+    ctl->fix_key_buf = 2;
+    ctl->fix_idx_buf = 1;
+    ctl->overflow    = 0;
+  }
+}
+
+// Tiles of the second pass from the first pass's window ends: tile_first[d] = sum_{e<d} ceil(cnt6[e] / tile), tile t = (window d,
+// offset) reads rows [d * cap + offset, + min(tile, cnt6[d] - offset)); the last tile is flagged. Counts are clamped to cap, so an
+// overflowed window never sends a reader past its buffer. Entries past the last tile stay zero (zero_head).
+__global__ void range_est_tiles_kernel(const sort_ctl* ctl, uint32_t cap, int tile, uint2* __restrict__ tiles)
+{
+  __shared__ uint32_t s_wsum[RADIX / 32];
+  const int d = threadIdx.x;  // 256 threads
+  const uint32_t cnt = min(ctl->base[1][6][d] - (uint32_t)d * cap, cap);
+  const uint32_t nt = (cnt + (uint32_t)tile - 1) / (uint32_t)tile;
+  const uint32_t inc = warp_inclusive_sum(nt);
+  if ((d & 31) == 31) s_wsum[d >> 5] = inc;
+  __syncthreads();
+  uint32_t first = inc - nt, total = 0;
+  for (int w = 0; w < RADIX / 32; ++w) {
+    first += w < (d >> 5) ? s_wsum[w] : 0u;
+    total += s_wsum[w];
+  }
+  for (uint32_t k = 0; k < nt; ++k) {
+    const uint32_t off = k * (uint32_t)tile;
+    const uint32_t t = first + k;
+    tiles[t] = make_uint2((uint32_t)d * cap + off, min((uint32_t)tile, cnt - off) | (t + 1 == total ? 0x80000000u : 0u));
+  }
+}
+
+// The range tier's two one-sweep passes into estimated digit windows of `cap` rows (digit d of pass p owns rows [d * cap, (d + 1) *
+// cap) of its output), then range_sort_kernel from the second pass's windows into the dense output. k1 / k2 / v1 / v2 hold 256 * cap
+// rows each (v*: pairs only; v2 is the second pass's destination). Returns false when a window, a range or a bucket overflowed:
+// the output is then incomplete and the caller runs the exact plan.
+template <typename UK, typename Shape, typename VT, bool CARRY>
+bool run_est_range(const UK* raw_keys, UK* keys_out, UK* k1, UK* k2, int32_t* idx_out, int32_t* v1, int32_t* v2, int64_t n, uint32_t cap,
+                   int kind, UK desc_mask, bool pairs, const void* val_in, cudaStream_t stream)
+{
+  static_assert(sizeof(UK) == 8, "the estimated-base range tier sorts 64-bit keys");
+  constexpr int TILE = Shape::tile;
+  const int64_t ntiles = (n + TILE - 1) / TILE + RADIX;  // window ends add at most 256 partial tiles
+  // the look-back rows behind the tile table are read and written in 16-byte groups: keep them 256-byte aligned
+  const size_t table_bytes = (sizeof(uint2) * ntiles + 255) / 256 * 256;
+  const onesweep_passes<UK, Shape, VT, CARRY, false, false, true> passes(n, 2, 0, table_bytes, stream, RADIX);
+  {
+    static std::atomic<uint64_t> attr_done{0};
+    once_per_device(attr_done, [] {
+      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem()));
+    });
+  }
+  sort_ctl* const ctl = passes.ctl();
+  uint2* const tiles = static_cast<uint2*>(passes.tail());
+  passes.zero_head(stream);
+  B2_LAUNCH(range_est_plan_kernel, 1, RADIX, 0, stream, ctl, cap);
+  pass_args a{};
+  a.key_bufs[0] = raw_keys;
+  a.key_bufs[1] = k1;
+  a.key_bufs[2] = k2;
+  a.idx_bufs[0] = idx_out;
+  a.idx_bufs[1] = v2;
+  a.idx_bufs[2] = v1;
+  a.ctl = ctl;
+  a.kind = kind;
+  a.pairs = pairs ? 1 : 0;
+  a.val_in = val_in;
+  a.desc_mask = (uint64_t)desc_mask;
+  a.est_cap = cap;
+  a.pass = 6;
+  passes.run(a, 0, "onesweep", stream);
+  B2_LAUNCH(range_est_tiles_kernel, 1, RADIX, 0, stream, (const sort_ctl*)ctl, cap, TILE, tiles);
+  a.pass = 7;
+  a.est_tiles = tiles;
+  passes.run(a, 1, "onesweep", stream, RADIX);
+  a.key_bufs[1] = keys_out;  // the range sort's keys-only destination
+  dbuf bounds(sizeof(uint32_t) * 3 * RADIX * RADIX, stream);
+  {
+    prof_scope ps("range_bounds", stream);
+    B2_LAUNCH(range_est_bounds_kernel, RADIX, RADIX, 0, stream, a, cap, bounds.as<uint32_t>());
+  }
+  {
+    prof_scope ps("segment_fix", stream);  // the range sort
+    B2_LAUNCH((range_sort_kernel<VT, true>), RADIX * RADIX, RANGE_THREADS, range_sort_smem(), stream, a, bounds.as<const uint32_t>());
+  }
+  uint32_t overflow = 0;
+  B2_CUDA_TRY(cudaMemcpyAsync(&overflow, &ctl->overflow, sizeof(overflow), cudaMemcpyDeviceToHost, stream));
+  B2_CUDA_TRY(cudaStreamSynchronize(stream));
+  return overflow == 0;
+}
+
 // Sort `n` keys.
 //  raw_keys != nullptr : keys are the user's raw column (twiddled on load, implicit row ids)
 //  raw_keys == nullptr : keys are pre-twiddled in bufA with explicit row ids in idx buffer pre_idx_buf
@@ -1499,11 +1714,25 @@ int64_t hybrid_min_rows()
 template <typename UK, typename Shape, typename VT = uint32_t, bool CARRY = false, bool MIX = false>
 void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int32_t* idx_tmp, int32_t* idx_tmp2, int pre_idx_buf, int64_t n,
                    int kind, bool descending, bool pairs, cudaStream_t stream, int first_pass = 0, int last_pass = 7,
-                   bool keep_keys = false, const void* val_in = nullptr, uint32_t* top_digit_base_out = nullptr)
+                   bool keep_keys = false, const void* val_in = nullptr, uint32_t* top_digit_base_out = nullptr, uint32_t est_cap = 0,
+                   void* est_buf = nullptr)
 {
   constexpr int NP = sizeof(UK);
   const bool raw = raw_keys != nullptr;
   const UK desc_mask = descending ? ~UK(0) : UK(0);
+
+  // est_cap != 0 (est_range_capacity): the range tier with estimated bases first. Its windows hold 256 * est_cap rows: bufB and
+  // est_buf (keys-only), bufA, bufB, idx_tmp and est_buf (pairs) are that large. An overflow falls back to the exact plan below.
+  if constexpr (sizeof(UK) == 8 && !MIX) {
+    if (est_cap != 0 && raw && first_pass == 0 && last_pass >= NP - 1 && !keep_keys) {
+      const bool done =
+        pairs ? run_est_range<UK, Shape, VT, CARRY>(raw_keys, bufA, bufA, bufB, idx_out, static_cast<int32_t*>(est_buf), idx_tmp, n, est_cap,
+                                                    kind, desc_mask, true, val_in, stream)
+              : run_est_range<UK, Shape, VT, CARRY>(raw_keys, bufA, static_cast<UK*>(est_buf), bufB, nullptr, nullptr, nullptr, n, est_cap,
+                                                    kind, desc_mask, false, val_in, stream);
+      if (done) return;
+    }
+  }
 
   const onesweep_passes<UK, Shape, VT, CARRY, MIX> passes(n, NP, sizeof(uint32_t) * NP * RADIX, 0, stream);
   sort_ctl* const ctl = passes.ctl();
@@ -1651,16 +1880,18 @@ using key_tile = std::conditional_t<sizeof(UK) == 8, tile_384x16, tile_512x16>;
 
 template <typename UK>
 void run_radix(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int32_t* idx_tmp, int pre_idx_buf, int64_t n,
-               int kind, bool descending, bool pairs, cudaStream_t stream, int32_t* idx_tmp2 = nullptr)
+               int kind, bool descending, bool pairs, cudaStream_t stream, int32_t* idx_tmp2 = nullptr, uint32_t est_cap = 0,
+               void* est_buf = nullptr)
 {
-  run_radix_cfg<UK, key_tile<UK>>(raw_keys, bufA, bufB, idx_out, idx_tmp, idx_tmp2, pre_idx_buf, n, kind, descending, pairs, stream);
+  run_radix_cfg<UK, key_tile<UK>>(raw_keys, bufA, bufB, idx_out, idx_tmp, idx_tmp2, pre_idx_buf, n, kind, descending, pairs, stream, 0, 7,
+                                  false, nullptr, nullptr, est_cap, est_buf);
 }
 
 // The 64-bit key kernels are instantiated here, ahead of the narrower key types that the sort entry points below instantiate.
 // How nvcc inlines the device helpers shared by the histogram, finalize and gather kernels depends on the order in which the
 // kernels are instantiated; this order gives every kernel the code the sort was measured with.
 template void run_radix_cfg<uint64_t, tile_384x16>(const uint64_t*, uint64_t*, uint64_t*, int32_t*, int32_t*, int32_t*, int, int64_t, int, bool,
-                                                   bool, cudaStream_t, int, int, bool, const void*, uint32_t*);
+                                                   bool, cudaStream_t, int, int, bool, const void*, uint32_t*, uint32_t, void*);
 
 }  // namespace
 
@@ -1717,17 +1948,29 @@ __global__ void est_plan_kernel(sort_ctl* ctl, int pass, uint32_t cap)
   }
 }
 
-// counts[b] = sampled rows (every `stride`-th) whose mix64(key) has top byte b
-__global__ void __launch_bounds__(256) est_sample_kernel(const uint64_t* __restrict__ keys, int64_t n, int64_t stride, unsigned int* __restrict__ counts)
+// MIX: counts[b] = sampled rows (every `stride`-th) whose mix64(key) has top byte b. Otherwise the keys are twiddled as the sort's
+// passes twiddle them (kind, desc_mask) and counts[b] / counts[256 + b] count digit 7 / digit 6 = b.
+template <bool MIX = true>
+__global__ void __launch_bounds__(256) est_sample_kernel(const uint64_t* __restrict__ keys, int64_t n, int64_t stride, unsigned int* __restrict__ counts,
+                                                         int kind = 0, uint64_t desc_mask = 0)
 {
-  __shared__ unsigned int sh[RADIX];
-  sh[threadIdx.x] = 0;
+  constexpr int NC = MIX ? 1 : 2;
+  __shared__ unsigned int sh[NC * RADIX];
+  for (int c = 0; c < NC; ++c) sh[c * RADIX + threadIdx.x] = 0;
   __syncthreads();
   const int64_t m = (n + stride - 1) / stride;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x)
-    atomicAdd(&sh[(unsigned)(mix64(keys[i * stride]) >> 56)], 1u);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (int64_t)gridDim.x * blockDim.x) {
+    if constexpr (MIX) {
+      atomicAdd(&sh[(unsigned)(mix64(keys[i * stride]) >> 56)], 1u);
+    } else {
+      const uint64_t k = twiddle_rt<uint64_t>(keys[i * stride], kind, desc_mask);
+      atomicAdd(&sh[(unsigned)(k >> 56)], 1u);
+      atomicAdd(&sh[RADIX + (unsigned)((k >> 48) & 255u)], 1u);
+    }
+  }
   __syncthreads();
-  if (sh[threadIdx.x]) atomicAdd(&counts[threadIdx.x], sh[threadIdx.x]);
+  for (int c = 0; c < NC; ++c)
+    if (sh[c * RADIX + threadIdx.x]) atomicAdd(&counts[c * RADIX + threadIdx.x], sh[c * RADIX + threadIdx.x]);
 }
 
 template <typename VT>
@@ -1779,7 +2022,7 @@ uint32_t radix_partition_est_capacity(const uint64_t* keys, int64_t n, cudaStrea
   const int64_t m = (n + stride - 1) / stride;
   dbuf cnt(sizeof(unsigned int) * RADIX, stream);
   B2_CUDA_TRY(cudaMemsetAsync(cnt.ptr, 0, cnt.bytes, stream));
-  B2_LAUNCH(est_sample_kernel, num_sms() * 4, 256, 0, stream, keys, n, stride, cnt.as<unsigned int>());
+  B2_LAUNCH((est_sample_kernel<true>), num_sms() * 4, 256, 0, stream, keys, n, stride, cnt.as<unsigned int>(), 0, (uint64_t)0);
   unsigned int h[RADIX];
   B2_CUDA_TRY(cudaMemcpyAsync(h, cnt.ptr, sizeof(h), cudaMemcpyDeviceToHost, stream));
   B2_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -1918,6 +2161,68 @@ void range_partition_scatter(const b2_column_view& keys, const b2_column_view* v
 
 namespace {
 
+// B2_SORT_EST=0 / 1 (test hook): the range tier with estimated bases off / on at any size where it applies; B2_SORT_EST_CAP=<rows>
+// (test hook) sets its window size without sampling (small values force the overflow fallback).
+int est_env()
+{
+  static int v = [] {
+    const char* e = std::getenv("B2_SORT_EST");
+    return e ? (std::atoi(e) != 0 ? 1 : 0) : -1;
+  }();
+  return v;
+}
+
+// Rows per digit window of the range tier with estimated bases (run_est_range), or 0 for the exact plan. It applies where the range
+// tier is tried (64-bit raw keys, from RANGE_MIN_ROWS rows on), on one portion, and not where the NaN count is needed (row ids of
+// descending float keys). A strided sample of 2^20 keys, twiddled as the passes twiddle them, must show both top digits varying, an
+// expected range length n * coll6 * coll7 + 5 sigma within RANGE_CAP, and a worst digit share (max sampled count + 5 sigma of the
+// sampling noise, scaled to n) within the groupby's bound n / 256 * 1.25 + 4096; cap is that share rounded up to 16 rows, so that
+// window starts stay 16-byte aligned for the bulk tile loads, and no larger: the four window buffers hold 256 * cap rows each.
+template <typename UK>
+uint32_t est_range_capacity(const UK* raw_keys, int64_t n, int kind, bool descending, bool pairs, int tile, cudaStream_t stream)
+{
+  if constexpr (sizeof(UK) != 8) {
+    return 0;
+  } else {
+    const int force = est_env();
+    if (force == 0 || n < 2 || n > portion_rows(tile)) return 0;
+    if (pairs && kind == (int)key_kind::FLOAT && descending) return 0;
+    if (range_env() == 0 || hybrid_min_rows() == INT64_MAX) return 0;
+    if (force != 1 && (n < RANGE_MIN_ROWS || n < hybrid_min_rows())) return 0;
+    if (const char* e = std::getenv("B2_SORT_EST_CAP")) return (uint32_t)std::max(1, std::atoi(e));
+    const int64_t stride = std::max<int64_t>(1, n >> 20);
+    const int64_t m = (n + stride - 1) / stride;
+    dbuf cnt(sizeof(unsigned int) * 2 * RADIX, stream);
+    B2_CUDA_TRY(cudaMemsetAsync(cnt.ptr, 0, cnt.bytes, stream));
+    {
+      prof_scope ps("est_sample", stream);
+      const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((m + 255) / 256, num_sms() * 4));
+      B2_LAUNCH((est_sample_kernel<false>), grid, 256, 0, stream, reinterpret_cast<const uint64_t*>(raw_keys), n, stride, cnt.as<unsigned int>(),
+                kind, (uint64_t)(descending ? ~UK(0) : UK(0)));
+    }
+    unsigned int h[2 * RADIX];
+    B2_CUDA_TRY(cudaMemcpyAsync(h, cnt.ptr, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    B2_CUDA_TRY(cudaStreamSynchronize(stream));
+    unsigned int mx[2] = {0, 0};
+    double coll[2] = {0.0, 0.0};
+    for (int c = 0; c < 2; ++c)
+      for (int d = 0; d < RADIX; ++d) {
+        mx[c] = std::max(mx[c], h[c * RADIX + d]);
+        const double f = (double)h[c * RADIX + d] / (double)m;
+        coll[c] += f * f;
+      }
+    if (mx[0] >= (unsigned)m || mx[1] >= (unsigned)m) return 0;  // a top digit is constant in the sample
+    const double e = (double)n * coll[0] * coll[1];
+    if (e + 5.0 * std::sqrt(e) > (double)RANGE_CAP) return 0;
+    const double top = (double)std::max(mx[0], mx[1]);
+    const double worst = (top + 5.0 * std::sqrt(top) + 1.0) * ((double)n / (double)m);
+    if (worst > (double)(n / RADIX) * 1.25 + 4096.0) return 0;
+    const uint64_t cap = ((uint64_t)std::ceil(worst) + 15) / 16 * 16;
+    if (cap * RADIX >= 4000000000ull) return 0;
+    return (uint32_t)cap;
+  }
+}
+
 int kind_of(int32_t storage_id)
 {
   if (is_float_id(storage_id)) return (int)key_kind::FLOAT;
@@ -1936,8 +2241,12 @@ column_ptr sorted_order_single(const b2_column_view& col, bool ascending, bool n
   int32_t* out_idx = out->data.as<int32_t>();
 
   if (!has_nulls(col)) {
-    dbuf a(sizeof(UK) * n, stream), b(sizeof(UK) > 1 ? sizeof(UK) * n : 0, stream), it(sizeof(int32_t) * n, stream);
-    run_radix<UK>(data, a.as<UK>(), b.as<UK>(), out_idx, it.as<int32_t>(), 0, n, kind, !ascending, true, stream);
+    // estimated-base range tier: the temporaries are its windows (256 * cap rows), also for the exact plan it falls back to
+    const uint32_t cap = est_range_capacity<UK>(data, n, kind, !ascending, true, key_tile<UK>::tile, stream);
+    const int64_t rows = cap ? std::max<int64_t>(n, (int64_t)RADIX * cap) : n;
+    dbuf a(sizeof(UK) * rows, stream), b(sizeof(UK) > 1 ? sizeof(UK) * rows : 0, stream), it(sizeof(int32_t) * rows, stream);
+    dbuf ev(cap ? sizeof(int32_t) * RADIX * (size_t)cap : 0, stream);
+    run_radix<UK>(data, a.as<UK>(), b.as<UK>(), out_idx, it.as<int32_t>(), 0, n, kind, !ascending, true, stream, nullptr, cap, ev.ptr);
     return out;
   }
   // nullable: nulls first iff (null_order == BEFORE) xor descending (sort_column_impl.cuh:35-57)
@@ -2149,17 +2458,21 @@ column_ptr sort_by_key_carry(const b2_column_view& keys, const b2_column_view& v
   const int kind = kind_of(storage_type(keys.type_id));
   auto out = make_column(values.type_id, (int32_t)n, false, stream);
   const int vw = type_width(values.type_id);
-  dbuf vtmp((size_t)vw * n, stream);
   const void* vin = static_cast<const char*>(values.data) + (size_t)values.offset * vw;
   auto go = [&](auto ktag, auto vtag) {
     using UK = decltype(ktag);
     using VT = decltype(vtag);
-    dbuf a(sizeof(UK) * n, stream), b(sizeof(UK) > 1 ? sizeof(UK) * n : 0, stream);
     // 8-byte payloads on 8-byte keys: 512 x 20 tiles, one CTA per SM, keys by one bulk async copy per tile: 13.2 instead of
     // 16.0 ms per 1e9-row pass on the H100 (DESIGN.md §4.1)
     using Shape = std::conditional_t<sizeof(UK) == 8 && sizeof(VT) == 8, tile_512x20_bulk, key_tile<UK>>;
-    run_radix_cfg<UK, Shape, VT, true>(static_cast<const UK*>(keys.data) + keys.offset, a.as<UK>(), b.as<UK>(), out->data.as<int32_t>(),
-                                       vtmp.as<int32_t>(), nullptr, 0, n, kind, !ascending, true, stream, 0, 7, false, vin);
+    const UK* kin = static_cast<const UK*>(keys.data) + keys.offset;
+    // estimated-base range tier: the temporaries are its windows (256 * cap rows), also for the exact plan it falls back to
+    const uint32_t cap = est_range_capacity<UK>(kin, n, kind, !ascending, true, Shape::tile, stream);
+    const int64_t rows = cap ? std::max<int64_t>(n, (int64_t)RADIX * cap) : n;
+    dbuf vtmp((size_t)vw * rows, stream), a(sizeof(UK) * rows, stream), b(sizeof(UK) > 1 ? sizeof(UK) * rows : 0, stream);
+    dbuf ev(cap ? (size_t)vw * RADIX * cap : 0, stream);
+    run_radix_cfg<UK, Shape, VT, true>(kin, a.as<UK>(), b.as<UK>(), out->data.as<int32_t>(), vtmp.as<int32_t>(), nullptr, 0, n, kind, !ascending,
+                                       true, stream, 0, 7, false, vin, nullptr, cap, ev.ptr);
   };
   auto by_key = [&](auto vtag) {
     switch (type_width(keys.type_id)) {
@@ -2184,9 +2497,12 @@ column_ptr sort_single_column(const b2_column_view& col, bool ascending, cudaStr
   B2_EXPECTS(kind != (int)key_kind::FLOAT, B2_ERR_LOGIC, "keys-only radix path is for integer-like keys");
   auto run = [&](auto tag) {
     using UK = decltype(tag);
-    dbuf tmp(sizeof(UK) > 1 ? sizeof(UK) * n : 0, stream);
-    run_radix<UK>(static_cast<const UK*>(col.data) + col.offset, out->data.as<UK>(), tmp.as<UK>(), nullptr, nullptr, 0, n, kind,
-                  !ascending, false, stream);
+    const UK* kin = static_cast<const UK*>(col.data) + col.offset;
+    // estimated-base range tier: the temporary and a second key buffer are its windows (256 * cap rows)
+    const uint32_t cap = est_range_capacity<UK>(kin, n, kind, !ascending, false, key_tile<UK>::tile, stream);
+    const int64_t rows = cap ? std::max<int64_t>(n, (int64_t)RADIX * cap) : n;
+    dbuf tmp(sizeof(UK) > 1 ? sizeof(UK) * rows : 0, stream), ev(cap ? sizeof(UK) * RADIX * (size_t)cap : 0, stream);
+    run_radix<UK>(kin, out->data.as<UK>(), tmp.as<UK>(), nullptr, nullptr, 0, n, kind, !ascending, false, stream, nullptr, cap, ev.ptr);
   };
   switch (type_width(col.type_id)) {
     case 1: run(uint8_t{}); break;

@@ -1141,12 +1141,15 @@ constexpr int RANGE_IPT         = RANGE_CAP / RANGE_THREADS;  // local row ids f
 constexpr int RANGE_BUCKET_BITS = 13;
 constexpr int RANGE_BUCKETS     = 1 << RANGE_BUCKET_BITS;
 constexpr int RANGE_BUCKET_CAP  = FIX_HALO;  // rows of one bucket: each row compares its key with all of them
+constexpr int RANGE_SLOTS       = RANGE_BUCKETS + RANGE_BUCKETS / 16;  // padded counter layout of range_sort_kernel<VT, true>
 
-size_t range_sort_smem()
+size_t range_sort_smem(bool est)
 {
   // scratch (mbarriers, overflow flag, scan) + keys, later the payload (one row of slack in front for the 16-byte aligned bulk
-  // copy) + bucket counters + local row ids grouped by bucket, then in sorted order
-  return 128 + sizeof(uint64_t) * (RANGE_CAP + 2) + sizeof(uint32_t) * RANGE_BUCKETS + sizeof(uint16_t) * RANGE_CAP;
+  // copy) + bucket counters + local row ids grouped by bucket (with estimated windows: and a 16-bit key digest), then in sorted
+  // order. With estimated windows that is 231 568 bytes, within the 232 448 one CTA may have.
+  return 128 + sizeof(uint64_t) * (RANGE_CAP + 2) +
+         (est ? sizeof(uint32_t) * (RANGE_SLOTS + RANGE_CAP) : sizeof(uint32_t) * RANGE_BUCKETS + sizeof(uint16_t) * RANGE_CAP);
 }
 
 // bounds[i] = first row of range i in the keys the last executed pass wrote, bounds[nranges] = n. One thread per range: a
@@ -1228,16 +1231,56 @@ __global__ void __launch_bounds__(RADIX) range_est_bounds_kernel(pass_args a, ui
   est[2 * R + i] = dense + lo;
 }
 
+// Phase probe of range_sort_kernel (scripts/range_probe.py), compiled only with -DB2_RANGE_PROBE: thread 0 of CTA i writes
+// clock64() at each phase boundary to g_range_probe[phase][i], its SM id and its row count behind them. The shipped build has
+// none of it (its SASS is the same with and without this block).
+#ifdef B2_RANGE_PROBE
+constexpr int RANGE_PROBE_CTAS   = 1 << 17;
+constexpr int RANGE_PROBE_STAMPS = 8;  // entry, keys waited, histogram, scan, scatter, walk, payload waited, write issued
+__device__ long long g_range_probe[RANGE_PROBE_STAMPS + 2][RANGE_PROBE_CTAS];
+void* g_range_probe_ptr()
+{
+  void* p = nullptr;
+  cudaGetSymbolAddress(&p, g_range_probe);
+  return p;
+}
+#define RANGE_PROBE_STAMP(i)                                                                  \
+  do {                                                                                        \
+    if (threadIdx.x == 0 && blockIdx.x < RANGE_PROBE_CTAS) g_range_probe[i][blockIdx.x] = clock64(); \
+  } while (0)
+#define RANGE_PROBE_SYNC() __syncthreads()
+#else
+#define RANGE_PROBE_STAMP(i) do {} while (0)
+#define RANGE_PROBE_SYNC() do {} while (0)
+#endif
+
+// #{rows of bucket positions [start, end) with a smaller (key, local row) than (k, r)}
+__device__ __attribute__((noinline)) uint32_t range_rank_keys(const uint32_t* s_ord, const uint64_t* sk, uint32_t start, uint32_t end,
+                                                              uint32_t r, uint64_t k)
+{
+  uint32_t before = 0;
+  for (uint32_t q = start; q < end; ++q) {
+    const uint32_t rq = s_ord[q] & 0xffffu;
+    const uint64_t kq = sk[rq];
+    before += (kq < k || (kq == k && rq < r)) ? 1u : 0u;
+  }
+  return before;
+}
+
 template <typename VT, bool EST = false>
 __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
 {
+  RANGE_PROBE_STAMP(0);
   using UK = uint64_t;
   B2_DYNAMIC_SMEM(smem_raw);
   uint32_t* s_misc = reinterpret_cast<uint32_t*>(smem_raw);                 // [0..1] / [2..3] key / payload mbarrier, [4] overflow, [16..31] scan
   UK* s_keys       = reinterpret_cast<UK*>(smem_raw + 128);                  // [RANGE_CAP + 2]
   VT* s_vals       = reinterpret_cast<VT*>(s_keys);                          // the payload window once the keys are dead
   uint32_t* s_cnt  = reinterpret_cast<uint32_t*>(s_keys + RANGE_CAP + 2);   // [RANGE_BUCKETS] bucket counters
-  uint16_t* s_perm = reinterpret_cast<uint16_t*>(s_cnt + RANGE_BUCKETS);    // [RANGE_CAP] local rows by bucket, then sorted
+  uint16_t* s_perm = reinterpret_cast<uint16_t*>(s_cnt + (EST ? RANGE_SLOTS : RANGE_BUCKETS));  // [RANGE_CAP] local rows by
+                                                                                                // bucket, then sorted
+  // estimated windows: the bucket order holds (digest << 16 | local row) in 32 bits, [RANGE_CAP]; s_perm aliases its front
+  uint32_t* s_ord  = reinterpret_cast<uint32_t*>(s_perm);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int64_t s = bounds[blockIdx.x];
@@ -1254,14 +1297,25 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     if (tid == 0) atomicOr(&a.ctl->overflow, 1u);
     return;
   }
+#ifdef B2_RANGE_PROBE
+  if (tid == 0 && blockIdx.x < RANGE_PROBE_CTAS) {
+    unsigned smid;
+    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+    g_range_probe[RANGE_PROBE_STAMPS][blockIdx.x]     = smid;
+    g_range_probe[RANGE_PROBE_STAMPS + 1][blockIdx.x] = m;
+  }
+#endif
   const UK* __restrict__ keys = static_cast<const UK*>(a.ctl->fix_key_buf == 1 ? a.key_bufs[1] : a.key_bufs[2]) + s;
   const VT* __restrict__ vin  = reinterpret_cast<const VT*>(a.ctl->fix_idx_buf == 1 ? a.idx_bufs[1] : a.idx_bufs[2]) + s;
   VT* __restrict__ vout = reinterpret_cast<VT*>(a.idx_bufs[0]) + o;
   UK* __restrict__ kout = static_cast<UK*>(const_cast<void*>(a.key_bufs[1])) + o;
 
   // bucket = the nb bits below the highest bit under the range id that varies over the input (bits between it and the range id
-  // are the same in every key); nb ~ log2 m, at most RANGE_BUCKET_BITS. Counter of bucket b: slot (b mod per) * RANGE_THREADS +
-  // b / per, so that thread t scans the `per` consecutive buckets t * per + j at conflict-free slots j * RANGE_THREADS + t.
+  // are the same in every key); nb ~ log2 m, at most RANGE_BUCKET_BITS. Thread t scans the `per` consecutive buckets t * per + j.
+  // Counter of bucket b, exact plan: slot (b mod per) * RANGE_THREADS + b / per, so the scan reads conflict-free slots
+  // j * RANGE_THREADS + t; but the walk's lookups of consecutive buckets then all hit one or two banks (16-way conflicts at
+  // per = 16). Estimated windows: slot b + b / per (one pad word behind every thread's buckets; b + b / 32 at per = 1), so the
+  // scan reads at a stride of per + 1 words and the walk's consecutive buckets sit in consecutive banks, both conflict-free.
   const uint64_t below = a.ctl->vary & ((1ull << a.ctl->range_shift) - 1);
   const uint32_t vhi = (uint32_t)(below >> 32), vlo = (uint32_t)below;
   const int top = vhi ? 64 - __clz((int)vhi) : (vlo ? 32 - __clz((int)vlo) : 0);  // bits [0, top) may differ within a range
@@ -1272,7 +1326,19 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   const int lp = max(nb - 9, 0);  // log2 per; RANGE_THREADS = 2^9
   const int per = 1 << lp;
   auto bucket = [&](UK k) { return (uint32_t)(k >> bshift) & bmask; };
-  auto slot   = [&](uint32_t b) { return ((b & (uint32_t)(per - 1)) << 9) | (b >> lp); };
+  // Keys of one bucket agree on every bit from bshift up, so the 16 bits below bshift (or bits [0, 16)) order two of them unless
+  // they are equal: the walk then compares the whole keys.
+  const int dshift = max(bshift - 16, 0);
+  auto digest = [&](UK k) { return (uint32_t)(k >> dshift) << 16; };
+  const int pad = lp ? lp : 5;
+  auto slot = [&](uint32_t b) {
+    if constexpr (EST) return b + (b >> pad);
+    else return ((b & (uint32_t)(per - 1)) << 9) | (b >> lp);
+  };
+  auto own = [&](int j) {  // slot of this thread's bucket j of the scan
+    if constexpr (EST) return (int)slot((uint32_t)(tid * per + j));
+    else return (j << 9) | tid;
+  };
 
   const uint32_t mbar_k = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc);
   const uint32_t mbar_v = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc + 2);
@@ -1283,7 +1349,8 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     }
   }
   if (tid == 0) s_misc[4] = 0;
-  for (int i = tid; i <= (int)bmask; i += RANGE_THREADS) s_cnt[i] = 0;
+  const int last = EST ? (int)slot(bmask) : (int)bmask;
+  for (int i = tid; i <= last; i += RANGE_THREADS) s_cnt[i] = 0;
   __syncthreads();
 
   // ---- keys -> s_keys; the payload window is written in sorted order at the end: bring it into L2 meanwhile ---------------
@@ -1297,17 +1364,19 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     if (kw.bulk) mbar_wait_phase0(mbar_k);
   }
   __syncthreads();
+  RANGE_PROBE_STAMP(1);
   const UK* sk = s_keys + kw.base;
 
   // ---- 1. counting pass: bucket histogram, exclusive scan (overflow check), scatter of the local rows ---------------------
   for (int r = tid; r < m; r += RANGE_THREADS) atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u);
   __syncthreads();
+  RANGE_PROBE_STAMP(2);
   uint32_t c[1 << (RANGE_BUCKET_BITS - 9)];
   uint32_t tot = 0;
   bool big = false;
 #pragma unroll
   for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
-    c[j] = (j < per && tid <= (int)bmask) ? s_cnt[(j << 9) | tid] : 0u;
+    c[j] = (j < per && tid <= (int)bmask) ? s_cnt[own(j)] : 0u;
     tot += c[j];
     big = big || c[j] > (uint32_t)RANGE_BUCKET_CAP;
   }
@@ -1324,13 +1393,22 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     for (int w = 0; w < warp; ++w) run += s_misc[16 + w];
 #pragma unroll
     for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
-      if (j < per && tid <= (int)bmask) s_cnt[(j << 9) | tid] = run;
+      if (j < per && tid <= (int)bmask) s_cnt[own(j)] = run;
       run += c[j];
     }
   }
   __syncthreads();
-  for (int r = tid; r < m; r += RANGE_THREADS) s_perm[atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u)] = (uint16_t)r;
+  RANGE_PROBE_STAMP(3);
+  if constexpr (EST) {
+    for (int r = tid; r < m; r += RANGE_THREADS) {
+      const UK k = sk[r];
+      s_ord[atomicAdd(&s_cnt[slot(bucket(k))], 1u)] = digest(k) | (uint32_t)r;
+    }
+  } else {
+    for (int r = tid; r < m; r += RANGE_THREADS) s_perm[atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u)] = (uint16_t)r;
+  }
   __syncthreads();
+  RANGE_PROBE_STAMP(4);
 
   // ---- 2. the row at bucket position p goes to bucket start + #{bucket rows with a smaller (key, local row)} --------------
   // (the counters now hold the bucket ends; consecutive positions share buckets, so a warp's walks are mostly broadcasts)
@@ -1339,20 +1417,41 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   for (int i = 0; i < RANGE_IPT; ++i) {
     const int p = tid + RANGE_THREADS * i;
     if (p >= m) break;
-    const uint32_t r = s_perm[p];
-    const UK k = sk[r];
-    const uint32_t b = bucket(k);
-    const uint32_t end = s_cnt[slot(b)];
-    const uint32_t start = b ? s_cnt[slot(b - 1)] : 0u;
-    uint32_t before = 0;
-    for (uint32_t q = start; q < end; ++q) {
-      const uint32_t rq = s_perm[q];
-      const UK kq = sk[rq];
-      before += (kq < k || (kq == k && rq < r)) ? 1u : 0u;
+    if constexpr (EST) {
+      // the bucket's entries are ranked by (digest, local row); only a bucket holding another row with the same digest is
+      // ranked again by whole keys (out of line: the unrolled walk must stay small enough for the instruction cache)
+      const uint32_t e = s_ord[p];
+      const uint32_t r = e & 0xffffu;
+      const UK k = sk[r];
+      const uint32_t b = bucket(k);
+      const uint32_t end = s_cnt[slot(b)];
+      const uint32_t start = b ? s_cnt[slot(b - 1)] : 0u;
+      uint32_t before = 0;
+      bool tie = false;
+      for (uint32_t q = start; q < end; ++q) {
+        const uint32_t eq = s_ord[q];
+        before += eq < e ? 1u : 0u;
+        tie = tie || ((eq ^ e) < 0x10000u && eq != e);
+      }
+      if (tie) before = range_rank_keys(s_ord, sk, start, end, r, k);
+      pk[i] = (start + before) | r << 16;
+    } else {
+      const uint32_t r = s_perm[p];
+      const UK k = sk[r];
+      const uint32_t b = bucket(k);
+      const uint32_t end = s_cnt[slot(b)];
+      const uint32_t start = b ? s_cnt[slot(b - 1)] : 0u;
+      uint32_t before = 0;
+      for (uint32_t q = start; q < end; ++q) {
+        const uint32_t rq = s_perm[q];
+        const UK kq = sk[rq];
+        before += (kq < k || (kq == k && rq < r)) ? 1u : 0u;
+      }
+      pk[i] = (start + before) | r << 16;
     }
-    pk[i] = (start + before) | r << 16;
   }
   __syncthreads();  // the keys (pairs) and the bucket order in s_perm are dead
+  RANGE_PROBE_STAMP(5);
 
   // ---- 3. sorted local rows -> s_perm; rows written in order from shared memory ----------------------------------------------
   range_window vw{0, false};
@@ -1366,6 +1465,7 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     if (vw.bulk) mbar_wait_phase0(mbar_v);
   }
   __syncthreads();
+  RANGE_PROBE_STAMP(6);
   if (a.pairs) {
     const VT* sv = s_vals + vw.base;
     for (int r = tid; r < m; r += RANGE_THREADS) vout[r] = sv[s_perm[r]];
@@ -1373,6 +1473,8 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     const UK desc = (UK)a.desc_mask;
     for (int r = tid; r < m; r += RANGE_THREADS) kout[r] = untwiddle_rt<UK>(sk[s_perm[r]], a.kind, desc);
   }
+  RANGE_PROBE_SYNC();
+  RANGE_PROBE_STAMP(7);
 }
 
 // descending float keys: cub sorts the (nan_bias, value) tuple descending, i.e. NaNs come first in
@@ -1665,7 +1767,7 @@ bool run_est_range(const UK* raw_keys, UK* keys_out, UK* k1, UK* k2, int32_t* id
   {
     static std::atomic<uint64_t> attr_done{0};
     once_per_device(attr_done, [] {
-      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem()));
+      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem(true)));
     });
   }
   sort_ctl* const ctl = passes.ctl();
@@ -1699,7 +1801,7 @@ bool run_est_range(const UK* raw_keys, UK* keys_out, UK* k1, UK* k2, int32_t* id
   }
   {
     prof_scope ps("segment_fix", stream);  // the range sort
-    B2_LAUNCH((range_sort_kernel<VT, true>), RADIX * RADIX, RANGE_THREADS, range_sort_smem(), stream, a, bounds.as<const uint32_t>());
+    B2_LAUNCH((range_sort_kernel<VT, true>), RADIX * RADIX, RANGE_THREADS, range_sort_smem(true), stream, a, bounds.as<const uint32_t>());
   }
   uint32_t overflow = 0;
   B2_CUDA_TRY(cudaMemcpyAsync(&overflow, &ctl->overflow, sizeof(overflow), cudaMemcpyDeviceToHost, stream));
@@ -1740,7 +1842,7 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
   if constexpr (sizeof(UK) == 8 && !MIX) {
     static std::atomic<uint64_t> attr_done{0};
     once_per_device(attr_done, [] {
-      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem()));
+      B2_CUDA_TRY(cudaFuncSetAttribute(range_sort_kernel<VT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)range_sort_smem(false)));
     });
   }
 
@@ -1843,7 +1945,7 @@ void run_radix_cfg(const UK* raw_keys, UK* bufA, UK* bufB, int32_t* idx_out, int
           B2_LAUNCH(range_bounds_kernel, (nranges + 256) / 256, 256, 0, stream, a, n, bounds.as<uint32_t>(), nranges);
         }
         prof_scope ps("segment_fix", stream);  // the range sort replaces the segment fix-up
-        B2_LAUNCH((range_sort_kernel<VT>), nranges, RANGE_THREADS, range_sort_smem(), stream, a, bounds.as<const uint32_t>());
+        B2_LAUNCH((range_sort_kernel<VT>), nranges, RANGE_THREADS, range_sort_smem(false), stream, a, bounds.as<const uint32_t>());
       } else if (try_hybrid && plan_hybrid) {
         const int64_t ntiles = (n + FIX_TILE - 1) / FIX_TILE;
         const int grid = (int)std::min<int64_t>(ntiles, num_sms() * 8);
@@ -2515,3 +2617,19 @@ column_ptr sort_single_column(const b2_column_view& col, bool ascending, cudaStr
 }
 
 }  // namespace b2
+
+#ifdef B2_RANGE_PROBE
+// scripts/range_probe.py: clears / copies out the phase stamps of the last range_sort_kernel launches (row-major
+// [RANGE_PROBE_STAMPS + 2][RANGE_PROBE_CTAS] int64).
+extern "C" B2_API int b2_range_probe_reset(void)
+{
+  return (int)cudaMemset(b2::g_range_probe_ptr(), 0, sizeof(long long) * (b2::RANGE_PROBE_STAMPS + 2) * b2::RANGE_PROBE_CTAS);
+}
+extern "C" B2_API int b2_range_probe_read(long long* out, int* stamps, int* ctas)
+{
+  *stamps = b2::RANGE_PROBE_STAMPS;
+  *ctas   = b2::RANGE_PROBE_CTAS;
+  return (int)cudaMemcpy(out, b2::g_range_probe_ptr(), sizeof(long long) * (b2::RANGE_PROBE_STAMPS + 2) * b2::RANGE_PROBE_CTAS,
+                         cudaMemcpyDeviceToHost);
+}
+#endif

@@ -144,6 +144,13 @@ _sig("b2_binary_operation", [P(ColumnView), P(ColumnView), i32, i32, b2_stream, 
 _sig("b2_binary_operation_cs", [P(ColumnView), vp, i32, i32, b2_stream, P(vp)])
 _sig("b2_binary_operation_sc", [vp, P(ColumnView), i32, i32, b2_stream, P(vp)])
 _sig("b2_binary_is_supported_operation", [i32, i32, i32, i32, P(i32)])
+_sig("b2_unary_operation", [P(ColumnView), i32, b2_stream, P(vp)])
+_sig("b2_cast", [P(ColumnView), i32, b2_stream, P(vp)])
+_sig("b2_is_supported_cast", [i32, i32, P(i32)])
+_sig("b2_is_null", [P(ColumnView), b2_stream, P(vp)])
+_sig("b2_is_valid", [P(ColumnView), b2_stream, P(vp)])
+_sig("b2_is_nan", [P(ColumnView), b2_stream, P(vp)])
+_sig("b2_is_not_nan", [P(ColumnView), b2_stream, P(vp)])
 _sig("b2_groupby_create", [P(TableView), i32, i32, u8p, i32, u8p, i32, P(vp)])
 _sig("b2_groupby_destroy", [vp], None)
 _sig("b2_groupby_aggregate", [vp, P(AggRequest), i32, b2_stream, P(vp), P(vp)])
@@ -198,7 +205,8 @@ DECLARED_SYMBOLS = [
     "b2_fill_splitmix64", "b2_apply_boolean_mask", "b2_drop_nulls", "b2_drop_nans", "b2_unique", "b2_distinct",
     "b2_distinct_indices", "b2_filtered_join_create", "b2_filtered_join_destroy", "b2_filtered_join_semi_join",
     "b2_filtered_join_anti_join", "b2_binary_operation", "b2_binary_operation_cs", "b2_binary_operation_sc",
-    "b2_binary_is_supported_operation",
+    "b2_binary_is_supported_operation", "b2_unary_operation", "b2_cast", "b2_is_supported_cast", "b2_is_null", "b2_is_valid",
+    "b2_is_nan", "b2_is_not_nan",
 ]
 
 

@@ -527,6 +527,94 @@ def is_supported_operation(out, lhs, rhs, op):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# unary operations and casts (python/pylibcudf/pylibcudf/unary.pyx; cpp/include/cudf/unary.hpp)
+# ---------------------------------------------------------------------------------------------------------------------
+def unary_operation(Column input, op, stream=None, mr=None):
+    """op(input[i]); the output type is the input's, INT32 for BIT_COUNT and BOOL8 for NOT."""
+    cdef int32_t o = int(op)
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_unary_operation(&input.v, o, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def cast(Column input, data_type, stream=None, mr=None):
+    """input converted to `data_type` (static_cast for numbers, chrono::floor between time units)."""
+    cdef int32_t t = int(data_type.id())
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_cast(&input.v, t, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def is_supported_cast(from_, to):
+    """Whether cast accepts this pair of types (cudf::is_supported_cast)."""
+    cdef int32_t r = 0
+    check(b2_is_supported_cast(int(from_.id()), int(to.id()), &r))
+    return r != 0
+
+
+def bit_cast(Column input, data_type, stream=None, mr=None):
+    """A new column of `data_type` holding a copy of input's bits and mask; both types fixed-width of the same storage width,
+    otherwise RuntimeError (cudf::logic_error)."""
+    from cudf_b200.pylibcudf.unary import _bit_castable
+    if not _bit_castable(input.type(), data_type):
+        raise RuntimeError(f"bit_cast: {input.type().id()!r} and {data_type.id()!r} are not bit-castable")
+    cdef b2_column_view v = input.v
+    v.type_id = int(data_type.id())  # the same bits seen as the target type: a same-type cast is a copy
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_cast(&v, v.type_id, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def _predicate(Column input, int which, stream):
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        if which == 0:
+            st = b2_is_null(&input.v, s, &out)
+        elif which == 1:
+            st = b2_is_valid(&input.v, s, &out)
+        elif which == 2:
+            st = b2_is_nan(&input.v, s, &out)
+        else:
+            st = b2_is_not_nan(&input.v, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def is_null(Column input, stream=None, mr=None):
+    """A BOOL8 column without a mask: True where input is null."""
+    return _predicate(input, 0, stream)
+
+
+def is_valid(Column input, stream=None, mr=None):
+    """A BOOL8 column without a mask: True where input is valid."""
+    return _predicate(input, 1, stream)
+
+
+def is_nan(Column input, stream=None, mr=None):
+    """A BOOL8 column without a mask: True where a FLOAT32 / FLOAT64 input is NaN (a null row is False)."""
+    return _predicate(input, 2, stream)
+
+
+def is_not_nan(Column input, stream=None, mr=None):
+    """A BOOL8 column without a mask: True where a FLOAT32 / FLOAT64 input is not NaN (a null row is True)."""
+    return _predicate(input, 3, stream)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # joins (python/pylibcudf/pylibcudf/join.pyx:63-205; cudf::hash_join)
 # ---------------------------------------------------------------------------------------------------------------------
 ctypedef b2_status (*free_join_fn)(const b2_table_view*, const b2_table_view*, int32_t, b2_stream, b2_column**, b2_column**) noexcept nogil

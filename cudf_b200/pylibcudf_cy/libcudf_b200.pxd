@@ -165,6 +165,15 @@ cdef extern from "cudf_b200.h" nogil:
                                      b2_column** out)
     b2_status b2_binary_is_supported_operation(int32_t out_type, int32_t lhs_type, int32_t rhs_type, int32_t op, int32_t* result)
 
+    # unary operations and casts (cpp/include/cudf/unary.hpp)
+    b2_status b2_unary_operation(const b2_column_view* input, int32_t op, b2_stream stream, b2_column** out)
+    b2_status b2_cast(const b2_column_view* input, int32_t out_type, b2_stream stream, b2_column** out)
+    b2_status b2_is_supported_cast(int32_t from_type, int32_t to_type, int32_t* result)
+    b2_status b2_is_null(const b2_column_view* input, b2_stream stream, b2_column** out)
+    b2_status b2_is_valid(const b2_column_view* input, b2_stream stream, b2_column** out)
+    b2_status b2_is_nan(const b2_column_view* input, b2_stream stream, b2_column** out)
+    b2_status b2_is_not_nan(const b2_column_view* input, b2_stream stream, b2_column** out)
+
     # cudf::pack / unpack (cpp/include/cudf/contiguous_split.hpp:233-317)
     void* b2_buffer_data(const b2_buffer* buf)
     size_t b2_buffer_size(const b2_buffer* buf)

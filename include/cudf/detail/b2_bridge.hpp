@@ -1025,4 +1025,91 @@ inline bool is_supported_operation(data_type out, data_type lhs, data_type rhs, 
 }
 }  // namespace binops
 
+// unary.hpp (cpp/include/cudf/unary.hpp:32-57,60-164): fixed-width columns; the semantics, undefined values and errors are
+// b2_unary_operation's and b2_cast's (include/cudf_b200.h).  An unsupported (op, type) pair, an op outside the enum, a
+// timestamp <-> numeric cast and a non-fixed-width cast target are cudf::logic_error; decimal, dictionary, string and nested
+// types cudf::data_type_error.  Deviation: is_supported_cast is false for decimal types (the reference casts them).
+enum class unary_operator : int32_t {
+  SIN, COS, TAN, ARCSIN, ARCCOS, ARCTAN, SINH, COSH, TANH, ARCSINH, ARCCOSH, ARCTANH, EXP, LOG, SQRT, CBRT, CEIL, FLOOR, ABS,
+  RINT, BIT_COUNT, BIT_INVERT, NOT, NEGATE
+};
+inline std::unique_ptr<column> unary_operation(column_view const& input, unary_operator op,
+                                               rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                               rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_unary_operation(&input.native(), static_cast<int32_t>(op), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> is_null(column_view const& input, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                       rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_is_null(&input.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> is_valid(column_view const& input, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                        rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_is_valid(&input.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> cast(column_view const& input, data_type out_type,
+                                    rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                    rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_cast(&input.native(), static_cast<int32_t>(out_type.id()), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline bool is_supported_cast(data_type from, data_type to) noexcept
+{
+  int32_t r = 0;
+  return b2_is_supported_cast(static_cast<int32_t>(from.id()), static_cast<int32_t>(to.id()), &r) == B2_OK && r != 0;
+}
+inline std::unique_ptr<column> is_nan(column_view const& input, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                      rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_is_nan(&input.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> is_not_nan(column_view const& input, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                          rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_is_not_nan(&input.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+
+// utilities/traits.hpp:681 and column/column_view.hpp:714-759: both types fixed-width with the same storage width (decimal
+// types are not held here, so none is bit-castable); bit_cast is a zero-copy view of the same data and mask
+namespace detail {
+constexpr int fixed_width_bytes(type_id t)
+{
+  switch (t) {
+    case type_id::INT8: case type_id::UINT8: case type_id::BOOL8: return 1;
+    case type_id::INT16: case type_id::UINT16: return 2;
+    case type_id::INT32: case type_id::UINT32: case type_id::FLOAT32: case type_id::TIMESTAMP_DAYS: case type_id::DURATION_DAYS:
+      return 4;
+    case type_id::INT64: case type_id::UINT64: case type_id::FLOAT64: case type_id::TIMESTAMP_SECONDS:
+    case type_id::TIMESTAMP_MILLISECONDS: case type_id::TIMESTAMP_MICROSECONDS: case type_id::TIMESTAMP_NANOSECONDS:
+    case type_id::DURATION_SECONDS: case type_id::DURATION_MILLISECONDS: case type_id::DURATION_MICROSECONDS:
+    case type_id::DURATION_NANOSECONDS: return 8;
+    default: return 0;
+  }
+}
+}  // namespace detail
+inline bool is_bit_castable(data_type from, data_type to)
+{
+  int const w = detail::fixed_width_bytes(from.id());
+  return w != 0 && w == detail::fixed_width_bytes(to.id());
+}
+inline column_view bit_cast(column_view const& input, data_type type)
+{
+  if (!is_bit_castable(input.type(), type)) throw cudf::logic_error("types are not bit-castable");
+  return column_view{type, input.size(), input.head<void>(), input.null_mask(), input.null_count(), input.offset()};
+}
+
 }  // namespace cudf

@@ -402,6 +402,56 @@ B2_API b2_status b2_binary_operation_sc(const b2_scalar* lhs, const b2_column_vi
 B2_API b2_status b2_binary_is_supported_operation(int32_t out_type, int32_t lhs_type, int32_t rhs_type, int32_t op,
                                                   int32_t* result);
 
+/* ---- unary operations and casts: cpp/include/cudf/unary.hpp, cpp/src/unary/{math_ops,cast_ops,nan_ops,null_ops}.cu -----------
+ * One elementwise pass over a fixed-width column.  The operator values are cudf::unary_operator's.  T is the input's type.
+ * b2_unary_operation:
+ *  - SIN .. ARCTANH, EXP, LOG, SQRT, CBRT, CEIL, FLOOR, ABS: INT8..UINT64, FLOAT32, FLOAT64, BOOL8 -> T.  FLOAT32 computes in
+ *    float, FLOAT64 in double, every integer type and BOOL8 in double and converts back to T (BOOL8: nonzero -> true).  No
+ *    fast-math: SQRT is correctly rounded, subnormals are kept.  ABS: signed integers abs() after integral promotion (INT8 -128
+ *    stays -128), unsigned integers and BOOL8 unchanged, floats fabs().
+ *  - RINT: FLOAT32, FLOAT64 -> T, half to even.
+ *  - BIT_COUNT: integer types and BOOL8 -> INT32, the popcount of the same-width unsigned value (BOOL8: 0 / 1).
+ *  - BIT_INVERT: integer types and BOOL8 -> T, ~x after promotion (BOOL8: every valid row true).
+ *  - NOT: INT8..BOOL8 -> BOOL8, x == 0 (NaN -> false, -0.0 -> true).
+ *  - NEGATE: signed integers, floats and every DURATION -> T, -x after promotion (floats flip the sign of +-0 and NaN).
+ * b2_cast (out_type any fixed-width id):
+ *  - numeric <-> numeric, BOOL8 included: static_cast (float -> integer truncates toward zero; -> BOOL8 is x != 0, NaN -> true);
+ *  - timestamp / duration <-> timestamp / duration: cuda::std::chrono::floor, ticks converted toward -inf in int64 and then
+ *    narrowed to the target's rep (int32 for DAYS, int64 otherwise);
+ *  - numeric -> duration: rep(x), a tick count with no unit scaling; duration -> numeric: To(count);
+ *  - a same-type cast is a copy.
+ * Null rows: the output has a mask exactly when the input has one (a copy of it, at offset 0), and the input's null_count.
+ * An empty input gives an empty column of the output type; b2_unary_operation then checks no type (RINT of an empty INT32
+ * column is an empty INT32 column).  No call synchronises.
+ * Undefined values (as in the reference; no result depends on them): float -> integer conversions of NaN or of a value whose
+ * truncation the target cannot hold (b2_cast, and the integer-typed results of the math operators: EXP of INT8 10, CEIL of
+ * INT64 near 2^63); ABS / NEGATE of INT32_MIN, INT64_MIN and the minimum duration; chrono up-casts that overflow int64 and
+ * down-casts whose result the int32 DAYS rep cannot hold; values under null bits.
+ * Errors: an unsupported (op, type) pair or an op outside the enum -> LOGIC; decimal, dictionary, string and nested inputs ->
+ * DATA_TYPE (the reference computes decimal ABS / CEIL / FLOOR / NEGATE; this library holds no decimal column).  b2_cast:
+ * timestamp <-> numeric -> LOGIC, even on an empty column; a decimal source or target -> DATA_TYPE; any other target that is
+ * not fixed-width -> LOGIC. */
+enum {
+  B2_UNARY_SIN = 0, B2_UNARY_COS = 1, B2_UNARY_TAN = 2, B2_UNARY_ARCSIN = 3, B2_UNARY_ARCCOS = 4, B2_UNARY_ARCTAN = 5,
+  B2_UNARY_SINH = 6, B2_UNARY_COSH = 7, B2_UNARY_TANH = 8, B2_UNARY_ARCSINH = 9, B2_UNARY_ARCCOSH = 10, B2_UNARY_ARCTANH = 11,
+  B2_UNARY_EXP = 12, B2_UNARY_LOG = 13, B2_UNARY_SQRT = 14, B2_UNARY_CBRT = 15, B2_UNARY_CEIL = 16, B2_UNARY_FLOOR = 17,
+  B2_UNARY_ABS = 18, B2_UNARY_RINT = 19, B2_UNARY_BIT_COUNT = 20, B2_UNARY_BIT_INVERT = 21, B2_UNARY_NOT = 22,
+  B2_UNARY_NEGATE = 23
+};
+B2_API b2_status b2_unary_operation(const b2_column_view* input, int32_t op, b2_stream stream, b2_column** out);
+B2_API b2_status b2_cast(const b2_column_view* input, int32_t out_type, b2_stream stream, b2_column** out);
+/* cudf::is_supported_cast: *result = 1 exactly when b2_cast accepts (from, to).  It equals the reference's answer on every pair
+ * of INT8..DURATION_NANOSECONDS; a decimal pair is 0 here (the reference supports decimal casts).  Type ids outside
+ * cudf::type_id -> LOGIC. */
+B2_API b2_status b2_is_supported_cast(int32_t from_type, int32_t to_type, int32_t* result);
+/* cudf::is_null / is_valid: a BOOL8 column without a mask, from the input's validity alone (any fixed-width type). */
+B2_API b2_status b2_is_null(const b2_column_view* input, b2_stream stream, b2_column** out);
+B2_API b2_status b2_is_valid(const b2_column_view* input, b2_stream stream, b2_column** out);
+/* cudf::is_nan / is_not_nan: FLOAT32 / FLOAT64 only (any other type -> LOGIC, even empty); a BOOL8 column without a mask, a
+ * null row is_nan = false and is_not_nan = true. */
+B2_API b2_status b2_is_nan(const b2_column_view* input, b2_stream stream, b2_column** out);
+B2_API b2_status b2_is_not_nan(const b2_column_view* input, b2_stream stream, b2_column** out);
+
 /* Two-phase form of b2_partition for the fused partition + exchange: the plan holds the bucket id and the
  * stable in-bucket rank of every row; out_counts[b] = rows of bucket b.  b2_partition_scatter then writes one
  * fixed-width column straight to P destination base addresses — local buffers or PEER device memory mapped with

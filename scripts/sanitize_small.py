@@ -52,4 +52,14 @@ plc.reduce.reduce(x, plc.aggregation.sum(), plc.DataType(plc.TypeId.INT64))
 t = plc.Table([kc, vc])
 plc.partitioning.hash_partition(t, [0], 13)
 plc.contiguous_split.unpack(plc.contiguous_split.pack(t))
+# unary operations and casts: vector and generic paths, a sliced view, is_null / is_nan
+xf = plc.Column.from_numpy(rng.normal(size=n), rng.random(n) < 0.9)
+plc.unary.unary_operation(xf, plc.unary.UnaryOperator.SQRT)
+plc.unary.unary_operation(xf.slice(3, n - 5), plc.unary.UnaryOperator.SIN)
+plc.unary.unary_operation(x, plc.unary.UnaryOperator.NEGATE)
+plc.unary.cast(x, plc.DataType(plc.TypeId.FLOAT64))
+plc.unary.cast(xf, plc.DataType(plc.TypeId.INT32))
+plc.unary.cast(plc.Column.from_numpy(k, dtype=plc.DataType(plc.TypeId.TIMESTAMP_NANOSECONDS)), plc.DataType(plc.TypeId.TIMESTAMP_DAYS))
+plc.unary.is_null(x.slice(1, n - 1))
+plc.unary.is_nan(xf)
 print("SANITIZE_SMALL_OK")

@@ -1135,20 +1135,30 @@ __global__ void __launch_bounds__(FIX_THREADS) segment_fix_kernel(pass_args a, i
 //      by a second bulk copy, and every output row is written coalesced from there.
 // A range longer than RANGE_CAP rows, or a bucket longer than RANGE_BUCKET_CAP rows (many equal or clustered keys), raises
 // ctl->overflow (the host reruns without the range tier).
-constexpr int RANGE_THREADS     = 512;
-constexpr int RANGE_WARPS       = RANGE_THREADS / 32;
-constexpr int RANGE_IPT         = RANGE_CAP / RANGE_THREADS;  // local row ids fit 16 bits
+// Threads per CTA: 2^9 on the exact plan, 2^10 with estimated windows. Either way one CTA fills an SM's shared memory; the
+// estimated-window kernel's walk is a chain of dependent shared-memory loads per row, and twice the warps overlap more of them.
+// The CPU emulator runs every thread of a CTA as a fiber, 65 536 CTAs per call, so there the kernel keeps 2^9 threads (its
+// code takes any 2^9 or 2^10) and the emulated tests keep their running time.
+template <bool EST>
+constexpr int range_log_threads = EST && !EMU_BUILD ? 10 : 9;
+constexpr int RANGE_THREADS     = 1 << range_log_threads<false>;
 constexpr int RANGE_BUCKET_BITS = 13;
 constexpr int RANGE_BUCKETS     = 1 << RANGE_BUCKET_BITS;
 constexpr int RANGE_BUCKET_CAP  = FIX_HALO;  // rows of one bucket: each row compares its key with all of them
-constexpr int RANGE_SLOTS       = RANGE_BUCKETS + RANGE_BUCKETS / 16;  // padded counter layout of range_sort_kernel<VT, true>
+constexpr int RANGE_SLOTS       = RANGE_BUCKETS + RANGE_BUCKETS / 32;  // padded counter layout of range_sort_kernel<VT, true>
+constexpr int RANGE_WALK_ROWS   = 4;  // rows of one thread whose bucket walks run side by side (estimated windows)
+// Estimated windows: a bucket order entry is (16-bit key digest << 15 | local row), local rows < RANGE_CAP = 2^14.
+constexpr uint32_t RANGE_ROW_MASK = (1u << 15) - 1;
+
+// Bytes in front of the keys: mbarriers, overflow flag and one scan word per warp from [16] on.
+constexpr int range_head_bytes(bool est) { return est ? 256 : 128; }
 
 size_t range_sort_smem(bool est)
 {
-  // scratch (mbarriers, overflow flag, scan) + keys, later the payload (one row of slack in front for the 16-byte aligned bulk
-  // copy) + bucket counters + local row ids grouped by bucket (with estimated windows: and a 16-bit key digest), then in sorted
-  // order. With estimated windows that is 231 568 bytes, within the 232 448 one CTA may have.
-  return 128 + sizeof(uint64_t) * (RANGE_CAP + 2) +
+  // scratch + keys, later the payload (one row of slack in front for the 16-byte aligned bulk copy) + bucket counters + local
+  // row ids grouped by bucket (with estimated windows: and a 16-bit key digest), then in sorted order. With estimated windows
+  // that is 230 672 bytes, within the 232 448 one CTA may have.
+  return range_head_bytes(est) + sizeof(uint64_t) * (RANGE_CAP + 2) +
          (est ? sizeof(uint32_t) * (RANGE_SLOTS + RANGE_CAP) : sizeof(uint32_t) * RANGE_BUCKETS + sizeof(uint16_t) * RANGE_CAP);
 }
 
@@ -1178,7 +1188,7 @@ struct range_window {
   int base;
   bool bulk;
 };
-template <typename T>
+template <int THREADS, typename T>
 __device__ __forceinline__ range_window range_window_load(T* sdst, const T* __restrict__ g, int64_t s, int m, uint32_t mbar)
 {
   constexpr int PER = 16 / sizeof(T);
@@ -1187,13 +1197,13 @@ __device__ __forceinline__ range_window range_window_load(T* sdst, const T* __re
   const int bulk_rows = bulk ? (m + off) / PER * PER : 0;
   if (bulk) {
     if constexpr (EMU_BUILD) {
-      for (int q = threadIdx.x; q < bulk_rows; q += RANGE_THREADS) sdst[q] = g[q - off];
+      for (int q = threadIdx.x; q < bulk_rows; q += THREADS) sdst[q] = g[q - off];
     } else {
       if (threadIdx.x == 0) bulk_copy_to_smem(sdst, g - off, (uint32_t)(sizeof(T) * bulk_rows), mbar);
     }
-    for (int r = bulk_rows - off + (int)threadIdx.x; r < m; r += RANGE_THREADS) sdst[off + r] = g[r];
+    for (int r = bulk_rows - off + (int)threadIdx.x; r < m; r += THREADS) sdst[off + r] = g[r];
   } else {
-    for (int q = threadIdx.x; q < m; q += RANGE_THREADS) sdst[q] = ld_stream(g + q);
+    for (int q = threadIdx.x; q < m; q += THREADS) sdst[q] = ld_stream(g + q);
   }
   return {bulk ? off : 0, bulk};
 }
@@ -1260,7 +1270,7 @@ __device__ __attribute__((noinline)) uint32_t range_rank_keys(const uint32_t* s_
 {
   uint32_t before = 0;
   for (uint32_t q = start; q < end; ++q) {
-    const uint32_t rq = s_ord[q] & 0xffffu;
+    const uint32_t rq = s_ord[q] & RANGE_ROW_MASK;
     const uint64_t kq = sk[rq];
     before += (kq < k || (kq == k && rq < r)) ? 1u : 0u;
   }
@@ -1268,18 +1278,21 @@ __device__ __attribute__((noinline)) uint32_t range_rank_keys(const uint32_t* s_
 }
 
 template <typename VT, bool EST = false>
-__global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
+__global__ void __launch_bounds__(1 << range_log_threads<EST>, 1) range_sort_kernel(pass_args a, const uint32_t* __restrict__ bounds)
 {
   RANGE_PROBE_STAMP(0);
   using UK = uint64_t;
+  constexpr int LT  = range_log_threads<EST>;
+  constexpr int RT  = 1 << LT;
+  constexpr int IPT = RANGE_CAP / RT;  // local row ids fit 16 bits
   B2_DYNAMIC_SMEM(smem_raw);
-  uint32_t* s_misc = reinterpret_cast<uint32_t*>(smem_raw);                 // [0..1] / [2..3] key / payload mbarrier, [4] overflow, [16..31] scan
-  UK* s_keys       = reinterpret_cast<UK*>(smem_raw + 128);                  // [RANGE_CAP + 2]
+  uint32_t* s_misc = reinterpret_cast<uint32_t*>(smem_raw);  // [0..1] / [2..3] key / payload mbarrier, [4] overflow, [16 + warp] scan
+  UK* s_keys       = reinterpret_cast<UK*>(smem_raw + range_head_bytes(EST));  // [RANGE_CAP + 2]
   VT* s_vals       = reinterpret_cast<VT*>(s_keys);                          // the payload window once the keys are dead
   uint32_t* s_cnt  = reinterpret_cast<uint32_t*>(s_keys + RANGE_CAP + 2);   // [RANGE_BUCKETS] bucket counters
   uint16_t* s_perm = reinterpret_cast<uint16_t*>(s_cnt + (EST ? RANGE_SLOTS : RANGE_BUCKETS));  // [RANGE_CAP] local rows by
                                                                                                 // bucket, then sorted
-  // estimated windows: the bucket order holds (digest << 16 | local row) in 32 bits, [RANGE_CAP]; s_perm aliases its front
+  // estimated windows: the bucket order holds (digest << 15 | local row) in 32 bits, [RANGE_CAP]; s_perm aliases its front
   uint32_t* s_ord  = reinterpret_cast<uint32_t*>(s_perm);
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1312,10 +1325,10 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
 
   // bucket = the nb bits below the highest bit under the range id that varies over the input (bits between it and the range id
   // are the same in every key); nb ~ log2 m, at most RANGE_BUCKET_BITS. Thread t scans the `per` consecutive buckets t * per + j.
-  // Counter of bucket b, exact plan: slot (b mod per) * RANGE_THREADS + b / per, so the scan reads conflict-free slots
-  // j * RANGE_THREADS + t; but the walk's lookups of consecutive buckets then all hit one or two banks (16-way conflicts at
-  // per = 16). Estimated windows: slot b + b / per (one pad word behind every thread's buckets; b + b / 32 at per = 1), so the
-  // scan reads at a stride of per + 1 words and the walk's consecutive buckets sit in consecutive banks, both conflict-free.
+  // Counter of bucket b, exact plan: slot (b mod per) * RT + b / per, so the scan reads conflict-free slots j * RT + t; but
+  // the walk's lookups of consecutive buckets then all hit one or two banks (16-way conflicts at per = 16). Estimated windows:
+  // slot b + b / 32 (one pad word behind every 32 buckets). The walk's consecutive buckets sit in consecutive banks, and for
+  // each per in {1, 2, 4, 8} the scan's reads of slots per * t + j by one warp fall in 32 distinct banks.
   const uint64_t below = a.ctl->vary & ((1ull << a.ctl->range_shift) - 1);
   const uint32_t vhi = (uint32_t)(below >> 32), vlo = (uint32_t)below;
   const int top = vhi ? 64 - __clz((int)vhi) : (vlo ? 32 - __clz((int)vlo) : 0);  // bits [0, top) may differ within a range
@@ -1323,21 +1336,20 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   const int nb = min(min(want, RANGE_BUCKET_BITS), top);
   const int bshift = top - nb;
   const uint32_t bmask = (1u << nb) - 1;
-  const int lp = max(nb - 9, 0);  // log2 per; RANGE_THREADS = 2^9
+  const int lp = max(nb - LT, 0);  // log2 per
   const int per = 1 << lp;
   auto bucket = [&](UK k) { return (uint32_t)(k >> bshift) & bmask; };
   // Keys of one bucket agree on every bit from bshift up, so the 16 bits below bshift (or bits [0, 16)) order two of them unless
   // they are equal: the walk then compares the whole keys.
   const int dshift = max(bshift - 16, 0);
-  auto digest = [&](UK k) { return (uint32_t)(k >> dshift) << 16; };
-  const int pad = lp ? lp : 5;
+  auto digest = [&](UK k) { return (uint32_t)(k >> dshift) << 15; };
   auto slot = [&](uint32_t b) {
-    if constexpr (EST) return b + (b >> pad);
-    else return ((b & (uint32_t)(per - 1)) << 9) | (b >> lp);
+    if constexpr (EST) return b + (b >> 5);
+    else return ((b & (uint32_t)(per - 1)) << LT) | (b >> lp);
   };
   auto own = [&](int j) {  // slot of this thread's bucket j of the scan
     if constexpr (EST) return (int)slot((uint32_t)(tid * per + j));
-    else return (j << 9) | tid;
+    else return (j << LT) | tid;
   };
 
   const uint32_t mbar_k = EMU_BUILD ? 0u : (uint32_t)__cvta_generic_to_shared(s_misc);
@@ -1350,11 +1362,11 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   }
   if (tid == 0) s_misc[4] = 0;
   const int last = EST ? (int)slot(bmask) : (int)bmask;
-  for (int i = tid; i <= last; i += RANGE_THREADS) s_cnt[i] = 0;
+  for (int i = tid; i <= last; i += RT) s_cnt[i] = 0;
   __syncthreads();
 
   // ---- keys -> s_keys; the payload window is written in sorted order at the end: bring it into L2 meanwhile ---------------
-  const range_window kw = range_window_load(s_keys, keys, s, m, mbar_k);
+  const range_window kw = range_window_load<RT>(s_keys, keys, s, m, mbar_k);
   if constexpr (!EMU_BUILD) {
     if (tid == 0 && a.pairs) {
       const uintptr_t lo = reinterpret_cast<uintptr_t>(vin) & ~uintptr_t(15);
@@ -1368,14 +1380,14 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   const UK* sk = s_keys + kw.base;
 
   // ---- 1. counting pass: bucket histogram, exclusive scan (overflow check), scatter of the local rows ---------------------
-  for (int r = tid; r < m; r += RANGE_THREADS) atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u);
+  for (int r = tid; r < m; r += RT) atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u);
   __syncthreads();
   RANGE_PROBE_STAMP(2);
-  uint32_t c[1 << (RANGE_BUCKET_BITS - 9)];
+  uint32_t c[1 << (RANGE_BUCKET_BITS - LT)];
   uint32_t tot = 0;
   bool big = false;
 #pragma unroll
-  for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
+  for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - LT)); ++j) {
     c[j] = (j < per && tid <= (int)bmask) ? s_cnt[own(j)] : 0u;
     tot += c[j];
     big = big || c[j] > (uint32_t)RANGE_BUCKET_CAP;
@@ -1392,7 +1404,7 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
     uint32_t run = inc - tot;
     for (int w = 0; w < warp; ++w) run += s_misc[16 + w];
 #pragma unroll
-    for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - 9)); ++j) {
+    for (int j = 0; j < (1 << (RANGE_BUCKET_BITS - LT)); ++j) {
       if (j < per && tid <= (int)bmask) s_cnt[own(j)] = run;
       run += c[j];
     }
@@ -1400,42 +1412,70 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   __syncthreads();
   RANGE_PROBE_STAMP(3);
   if constexpr (EST) {
-    for (int r = tid; r < m; r += RANGE_THREADS) {
+    for (int r = tid; r < m; r += RT) {
       const UK k = sk[r];
       s_ord[atomicAdd(&s_cnt[slot(bucket(k))], 1u)] = digest(k) | (uint32_t)r;
     }
   } else {
-    for (int r = tid; r < m; r += RANGE_THREADS) s_perm[atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u)] = (uint16_t)r;
+    for (int r = tid; r < m; r += RT) s_perm[atomicAdd(&s_cnt[slot(bucket(sk[r]))], 1u)] = (uint16_t)r;
   }
   __syncthreads();
   RANGE_PROBE_STAMP(4);
 
   // ---- 2. the row at bucket position p goes to bucket start + #{bucket rows with a smaller (key, local row)} --------------
   // (the counters now hold the bucket ends; consecutive positions share buckets, so a warp's walks are mostly broadcasts)
-  uint32_t pk[RANGE_IPT];  // destination | local row << 16
+  uint32_t pk[IPT];  // destination | local row << 16
+  if constexpr (EST) {
+    // A row's place in its bucket is the number of the bucket's entries with a smaller digest, unless another row shares its
+    // digest: that bucket is ranked again by whole keys (out of line: the unrolled walk must stay small enough for the
+    // instruction cache). Entries and the bounds lo / hi lie in [0, 2^31], so the sign bit of eq - lo (eq - hi) says whether
+    // eq's digest is smaller than (at most) this row's: one subtraction and one shift-add per count. The rows go in groups of
+    // RANGE_WALK_ROWS: the entry, key and counter loads of a group issue together, and one loop as long as the group's largest
+    // bucket walks its buckets side by side, each read clamped to its bucket's last entry, whose extra reads are subtracted
+    // behind the loop. Rows past m walk the one-entry bucket [0, 1) and are not written.
 #pragma unroll
-  for (int i = 0; i < RANGE_IPT; ++i) {
-    const int p = tid + RANGE_THREADS * i;
-    if (p >= m) break;
-    if constexpr (EST) {
-      // the bucket's entries are ranked by (digest, local row); only a bucket holding another row with the same digest is
-      // ranked again by whole keys (out of line: the unrolled walk must stay small enough for the instruction cache)
-      const uint32_t e = s_ord[p];
-      const uint32_t r = e & 0xffffu;
-      const UK k = sk[r];
-      const uint32_t b = bucket(k);
-      const uint32_t end = s_cnt[slot(b)];
-      const uint32_t start = b ? s_cnt[slot(b - 1)] : 0u;
-      uint32_t before = 0;
-      bool tie = false;
-      for (uint32_t q = start; q < end; ++q) {
-        const uint32_t eq = s_ord[q];
-        before += eq < e ? 1u : 0u;
-        tie = tie || ((eq ^ e) < 0x10000u && eq != e);
+    for (int i0 = 0; i0 < IPT; i0 += RANGE_WALK_ROWS) {
+      if (tid + RT * i0 >= m) break;
+      uint32_t e[RANGE_WALK_ROWS], start[RANGE_WALK_ROWS], end[RANGE_WALK_ROWS];
+#pragma unroll
+      for (int g = 0; g < RANGE_WALK_ROWS; ++g) e[g] = tid + RT * (i0 + g) < m ? s_ord[tid + RT * (i0 + g)] : 0u;
+      uint32_t len = 0;
+#pragma unroll
+      for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
+        const bool in = tid + RT * (i0 + g) < m;
+        const uint32_t b = bucket(sk[e[g] & RANGE_ROW_MASK]);
+        end[g] = in ? s_cnt[slot(b)] : 1u;
+        start[g] = in && b ? s_cnt[slot(b - 1)] : 0u;
+        len = max(len, end[g] - start[g]);
       }
-      if (tie) before = range_rank_keys(s_ord, sk, start, end, r, k);
-      pk[i] = (start + before) | r << 16;
-    } else {
+      // entries of a smaller digest lie below lo, of at most this row's digest below hi
+      auto lo = [&](int g) { return e[g] & ~RANGE_ROW_MASK; };
+      auto hi = [&](int g) { return (e[g] & ~RANGE_ROW_MASK) + RANGE_ROW_MASK + 1; };
+      uint32_t lt[RANGE_WALK_ROWS] = {}, le[RANGE_WALK_ROWS] = {};
+      for (uint32_t q = 0; q < len; ++q) {
+#pragma unroll
+        for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
+          const uint32_t eq = s_ord[min(start[g] + q, end[g] - 1)];
+          lt[g] += (eq - lo(g)) >> 31;
+          le[g] += (eq - hi(g)) >> 31;
+        }
+      }
+#pragma unroll
+      for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
+        const uint32_t extra = len - (end[g] - start[g]);
+        const uint32_t eq = s_ord[end[g] - 1];
+        lt[g] -= extra * ((eq - lo(g)) >> 31);
+        le[g] -= extra * ((eq - hi(g)) >> 31);
+        const uint32_t r = e[g] & RANGE_ROW_MASK;
+        if (le[g] - lt[g] > 1u) lt[g] = range_rank_keys(s_ord, sk, start[g], end[g], r, sk[r]);
+        pk[i0 + g] = (start[g] + lt[g]) | r << 16;
+      }
+    }
+  } else {
+#pragma unroll
+    for (int i = 0; i < IPT; ++i) {
+      const int p = tid + RT * i;
+      if (p >= m) break;
       const uint32_t r = s_perm[p];
       const UK k = sk[r];
       const uint32_t b = bucket(k);
@@ -1455,10 +1495,10 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
 
   // ---- 3. sorted local rows -> s_perm; rows written in order from shared memory ----------------------------------------------
   range_window vw{0, false};
-  if (a.pairs) vw = range_window_load(s_vals, vin, s, m, mbar_v);
+  if (a.pairs) vw = range_window_load<RT>(s_vals, vin, s, m, mbar_v);
 #pragma unroll
-  for (int i = 0; i < RANGE_IPT; ++i) {
-    if (tid + RANGE_THREADS * i >= m) break;
+  for (int i = 0; i < IPT; ++i) {
+    if (tid + RT * i >= m) break;
     s_perm[pk[i] & 0xffffu] = (uint16_t)(pk[i] >> 16);
   }
   if constexpr (!EMU_BUILD) {
@@ -1468,10 +1508,10 @@ __global__ void __launch_bounds__(RANGE_THREADS, 1) range_sort_kernel(pass_args 
   RANGE_PROBE_STAMP(6);
   if (a.pairs) {
     const VT* sv = s_vals + vw.base;
-    for (int r = tid; r < m; r += RANGE_THREADS) vout[r] = sv[s_perm[r]];
+    for (int r = tid; r < m; r += RT) vout[r] = sv[s_perm[r]];
   } else {
     const UK desc = (UK)a.desc_mask;
-    for (int r = tid; r < m; r += RANGE_THREADS) kout[r] = untwiddle_rt<UK>(sk[s_perm[r]], a.kind, desc);
+    for (int r = tid; r < m; r += RT) kout[r] = untwiddle_rt<UK>(sk[s_perm[r]], a.kind, desc);
   }
   RANGE_PROBE_SYNC();
   RANGE_PROBE_STAMP(7);
@@ -1801,7 +1841,7 @@ bool run_est_range(const UK* raw_keys, UK* keys_out, UK* k1, UK* k2, int32_t* id
   }
   {
     prof_scope ps("segment_fix", stream);  // the range sort
-    B2_LAUNCH((range_sort_kernel<VT, true>), RADIX * RADIX, RANGE_THREADS, range_sort_smem(true), stream, a, bounds.as<const uint32_t>());
+    B2_LAUNCH((range_sort_kernel<VT, true>), RADIX * RADIX, 1 << range_log_threads<true>, range_sort_smem(true), stream, a, bounds.as<const uint32_t>());
   }
   uint32_t overflow = 0;
   B2_CUDA_TRY(cudaMemcpyAsync(&overflow, &ctl->overflow, sizeof(overflow), cudaMemcpyDeviceToHost, stream));

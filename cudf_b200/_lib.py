@@ -151,6 +151,15 @@ _sig("b2_is_null", [P(ColumnView), b2_stream, P(vp)])
 _sig("b2_is_valid", [P(ColumnView), b2_stream, P(vp)])
 _sig("b2_is_nan", [P(ColumnView), b2_stream, P(vp)])
 _sig("b2_is_not_nan", [P(ColumnView), b2_stream, P(vp)])
+_sig("b2_replace_nulls", [P(ColumnView), P(ColumnView), b2_stream, P(vp)])
+_sig("b2_replace_nulls_scalar", [P(ColumnView), vp, b2_stream, P(vp)])
+_sig("b2_replace_nulls_policy", [P(ColumnView), i32, b2_stream, P(vp)])
+_sig("b2_replace_nans", [P(ColumnView), P(ColumnView), b2_stream, P(vp)])
+_sig("b2_replace_nans_scalar", [P(ColumnView), vp, b2_stream, P(vp)])
+_sig("b2_find_and_replace_all", [P(ColumnView), P(ColumnView), P(ColumnView), b2_stream, P(vp)])
+_sig("b2_clamp", [P(ColumnView), vp, vp, vp, vp, b2_stream, P(vp)])
+_sig("b2_normalize_nans_and_zeros", [P(ColumnView), b2_stream, P(vp)])
+_sig("b2_normalize_nans_and_zeros_inplace", [P(ColumnView), b2_stream])
 _sig("b2_groupby_create", [P(TableView), i32, i32, u8p, i32, u8p, i32, P(vp)])
 _sig("b2_groupby_destroy", [vp], None)
 _sig("b2_groupby_aggregate", [vp, P(AggRequest), i32, b2_stream, P(vp), P(vp)])
@@ -206,7 +215,9 @@ DECLARED_SYMBOLS = [
     "b2_distinct_indices", "b2_filtered_join_create", "b2_filtered_join_destroy", "b2_filtered_join_semi_join",
     "b2_filtered_join_anti_join", "b2_binary_operation", "b2_binary_operation_cs", "b2_binary_operation_sc",
     "b2_binary_is_supported_operation", "b2_unary_operation", "b2_cast", "b2_is_supported_cast", "b2_is_null", "b2_is_valid",
-    "b2_is_nan", "b2_is_not_nan",
+    "b2_is_nan", "b2_is_not_nan", "b2_replace_nulls", "b2_replace_nulls_scalar", "b2_replace_nulls_policy", "b2_replace_nans",
+    "b2_replace_nans_scalar", "b2_find_and_replace_all", "b2_clamp", "b2_normalize_nans_and_zeros",
+    "b2_normalize_nans_and_zeros_inplace",
 ]
 
 

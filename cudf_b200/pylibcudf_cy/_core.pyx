@@ -615,6 +615,84 @@ def is_not_nan(Column input, stream=None, mr=None):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# replacement (python/pylibcudf/pylibcudf/replace.pyx; cpp/include/cudf/replace.hpp)
+# ---------------------------------------------------------------------------------------------------------------------
+def replace_nulls(Column source_column, replacement, stream=None, mr=None):
+    """Nulls of source_column replaced: by replacement[i] (a Column), by one value (a Scalar; the output has no mask), or by the
+    nearest valid value before / after the row (a ReplacePolicy; a leading / trailing null run stays null)."""
+    from cudf_b200.pylibcudf.replace import ReplacePolicy
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    cdef Column rc
+    cdef const b2_scalar* sc
+    cdef int32_t policy
+    if isinstance(replacement, Column):
+        rc = replacement
+        with nogil:
+            st = b2_replace_nulls(&source_column.v, &rc.v, s, &out)
+    elif isinstance(replacement, _PlcScalar):
+        sc = <const b2_scalar*><uintptr_t>replacement._handle
+        with nogil:
+            st = b2_replace_nulls_scalar(&source_column.v, sc, s, &out)
+    elif isinstance(replacement, ReplacePolicy):
+        policy = int(replacement)
+        with nogil:
+            st = b2_replace_nulls_policy(&source_column.v, policy, s, &out)
+    else:
+        raise TypeError("replacement must be a Column, Scalar, or replace_policy")
+    check(st)
+    return Column.from_handle(out)
+
+
+def find_and_replace_all(Column source_column, Column values_to_replace, Column replacement_values, stream=None, mr=None):
+    """Rows equal to values_to_replace[j] take replacement_values[j] (the first j among duplicates; -0.0 == +0.0, NaN matches
+    nothing)."""
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_find_and_replace_all(&source_column.v, &values_to_replace.v, &replacement_values.v, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def clamp(Column source_column, lo, hi, lo_replace=None, hi_replace=None, stream=None, mr=None):
+    """x < lo -> lo_replace (default lo), x > hi -> hi_replace (default hi); a null bound is not applied."""
+    if (lo_replace is None) != (hi_replace is None):
+        raise ValueError("lo_replace and hi_replace must be specified together")
+    if lo_replace is None:
+        lo_replace, hi_replace = lo, hi
+    cdef const b2_scalar* l = <const b2_scalar*><uintptr_t>lo._handle
+    cdef const b2_scalar* lr = <const b2_scalar*><uintptr_t>lo_replace._handle
+    cdef const b2_scalar* h = <const b2_scalar*><uintptr_t>hi._handle
+    cdef const b2_scalar* hr = <const b2_scalar*><uintptr_t>hi_replace._handle
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        st = b2_clamp(&source_column.v, l, lr, h, hr, s, &out)
+    check(st)
+    return Column.from_handle(out)
+
+
+def normalize_nans_and_zeros(Column source_column, bint inplace=False, stream=None, mr=None):
+    """Every NaN as quiet_NaN() and -0.0 as +0.0 (FLOAT32 / FLOAT64). inplace=True rewrites source_column's data and returns
+    None."""
+    cdef b2_stream s = _stream(stream)
+    cdef b2_column* out = NULL
+    cdef b2_status st
+    with nogil:
+        if inplace:
+            st = b2_normalize_nans_and_zeros_inplace(&source_column.v, s)
+        else:
+            st = b2_normalize_nans_and_zeros(&source_column.v, s, &out)
+    check(st)
+    if not inplace:
+        return Column.from_handle(out)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # joins (python/pylibcudf/pylibcudf/join.pyx:63-205; cudf::hash_join)
 # ---------------------------------------------------------------------------------------------------------------------
 ctypedef b2_status (*free_join_fn)(const b2_table_view*, const b2_table_view*, int32_t, b2_stream, b2_column**, b2_column**) noexcept nogil

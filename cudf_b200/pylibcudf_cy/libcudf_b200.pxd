@@ -174,6 +174,17 @@ cdef extern from "cudf_b200.h" nogil:
     b2_status b2_is_nan(const b2_column_view* input, b2_stream stream, b2_column** out)
     b2_status b2_is_not_nan(const b2_column_view* input, b2_stream stream, b2_column** out)
 
+    # replacement (cpp/include/cudf/replace.hpp)
+    b2_status b2_replace_nulls(const b2_column_view* input, const b2_column_view* replacement, b2_stream stream, b2_column** out)
+    b2_status b2_replace_nulls_scalar(const b2_column_view* input, const b2_scalar* replacement, b2_stream stream, b2_column** out)
+    b2_status b2_replace_nulls_policy(const b2_column_view* input, int32_t policy, b2_stream stream, b2_column** out)
+    b2_status b2_find_and_replace_all(const b2_column_view* input, const b2_column_view* values_to_replace,
+                                      const b2_column_view* replacement_values, b2_stream stream, b2_column** out)
+    b2_status b2_clamp(const b2_column_view* input, const b2_scalar* lo, const b2_scalar* lo_replace, const b2_scalar* hi,
+                       const b2_scalar* hi_replace, b2_stream stream, b2_column** out)
+    b2_status b2_normalize_nans_and_zeros(const b2_column_view* input, b2_stream stream, b2_column** out)
+    b2_status b2_normalize_nans_and_zeros_inplace(const b2_column_view* in_out, b2_stream stream)
+
     # cudf::pack / unpack (cpp/include/cudf/contiguous_split.hpp:233-317)
     void* b2_buffer_data(const b2_buffer* buf)
     size_t b2_buffer_size(const b2_buffer* buf)

@@ -166,7 +166,12 @@ class column_view {
  private:
   b2_column_view v_{};
 };
-using mutable_column_view = column_view;
+// a view whose data the callee may write (normalize_nans_and_zeros in place); a column_view otherwise
+class mutable_column_view : public column_view {
+ public:
+  using column_view::column_view;
+  template <typename T> [[nodiscard]] T* data() const noexcept { return const_cast<T*>(column_view::data<T>()); }
+};
 
 class table_view {
  public:
@@ -209,6 +214,12 @@ class column {
     return column_view{data_type{static_cast<type_id>(v.type_id)}, v.size, v.data, v.null_mask, v.null_count, v.offset};
   }
   operator column_view() const { return view(); }
+  [[nodiscard]] mutable_column_view mutable_view()
+  {
+    column_view const v = view();
+    return mutable_column_view{v.type(), v.size(), v.head<void>(), v.null_mask(), v.null_count(), v.offset()};
+  }
+  operator mutable_column_view() { return mutable_view(); }
   [[nodiscard]] data_type type() const { return view().type(); }
   [[nodiscard]] size_type size() const { return view().size(); }
   [[nodiscard]] size_type null_count() const { return view().null_count(); }
@@ -1110,6 +1121,88 @@ inline column_view bit_cast(column_view const& input, data_type type)
 {
   if (!is_bit_castable(input.type(), type)) throw cudf::logic_error("types are not bit-castable");
   return column_view{type, input.size(), input.head<void>(), input.null_mask(), input.null_count(), input.offset()};
+}
+
+// replace.hpp (cpp/include/cudf/replace.hpp): fixed-width columns; the semantics and errors are b2_replace_nulls*',
+// b2_replace_nans*', b2_find_and_replace_all's, b2_clamp's and b2_normalize_nans_and_zeros*' (include/cudf_b200.h).  LOGIC is
+// cudf::logic_error and DATA_TYPE cudf::data_type_error.
+enum class replace_policy : bool { PRECEDING, FOLLOWING };
+inline std::unique_ptr<column> replace_nulls(column_view const& input, column_view const& replacement,
+                                             rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                             rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_replace_nulls(&input.native(), &replacement.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> replace_nulls(column_view const& input, scalar const& replacement,
+                                             rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                             rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_replace_nulls_scalar(&input.native(), replacement.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> replace_nulls(column_view const& input, replace_policy const& policy,
+                                             rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                             rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_replace_nulls_policy(&input.native(), policy == replace_policy::PRECEDING ? B2_REPLACE_PRECEDING : B2_REPLACE_FOLLOWING,
+                                        stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> replace_nans(column_view const& input, column_view const& replacement,
+                                            rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                            rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_replace_nans(&input.native(), &replacement.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> replace_nans(column_view const& input, scalar const& replacement,
+                                            rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                            rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_replace_nans_scalar(&input.native(), replacement.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> find_and_replace_all(column_view const& input_col, column_view const& values_to_replace,
+                                                    column_view const& replacement_values,
+                                                    rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                    rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_find_and_replace_all(&input_col.native(), &values_to_replace.native(), &replacement_values.native(), stream.value(),
+                                        &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> clamp(column_view const& input, scalar const& lo, scalar const& lo_replace, scalar const& hi,
+                                     scalar const& hi_replace, rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                     rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_clamp(&input.native(), lo.native(), lo_replace.native(), hi.native(), hi_replace.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline std::unique_ptr<column> clamp(column_view const& input, scalar const& lo, scalar const& hi,
+                                     rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                     rmm::device_async_resource_ref mr = cudf::get_current_device_resource_ref())
+{
+  return clamp(input, lo, lo, hi, hi, stream, mr);
+}
+inline std::unique_ptr<column> normalize_nans_and_zeros(column_view const& input,
+                                                        rmm::cuda_stream_view stream = cudf::get_default_stream(),
+                                                        rmm::device_async_resource_ref = cudf::get_current_device_resource_ref())
+{
+  b2_column* out = nullptr;
+  detail::check(b2_normalize_nans_and_zeros(&input.native(), stream.value(), &out));
+  return std::make_unique<column>(out);
+}
+inline void normalize_nans_and_zeros(mutable_column_view& in_out, rmm::cuda_stream_view stream = cudf::get_default_stream())
+{
+  detail::check(b2_normalize_nans_and_zeros_inplace(&in_out.native(), stream.value()));
 }
 
 }  // namespace cudf

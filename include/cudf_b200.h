@@ -452,6 +452,48 @@ B2_API b2_status b2_is_valid(const b2_column_view* input, b2_stream stream, b2_c
 B2_API b2_status b2_is_nan(const b2_column_view* input, b2_stream stream, b2_column** out);
 B2_API b2_status b2_is_not_nan(const b2_column_view* input, b2_stream stream, b2_column** out);
 
+/* ---- replacement: cpp/include/cudf/replace.hpp, cpp/src/replace/{nulls,nans,replace,clamp}.cu -------------------------------
+ * One pass over a fixed-width column (INT8..DURATION_NANOSECONDS).  "A copy" is a new column with the input view's values, its
+ * mask (realigned to offset 0) when it has one, and its null count.  An empty input gives an empty column (find_and_replace_all,
+ * clamp, normalize: a copy) after the checks listed below.  Where the output's mask is computed, its null count is counted on
+ * the device (the column resolves it on first use); only the scalar forms of replace_nulls and clamp synchronise, to read the
+ * scalars' validity.
+ * b2_replace_nulls: out[i] = valid(in[i]) ? in[i] : replacement[i].  The output has a mask exactly when the replacement has
+ *   nulls.  An input without nulls gives a copy.  Errors: types differ -> DATA_TYPE; sizes differ -> LOGIC.
+ * b2_replace_nulls_scalar: null rows take the scalar; the output has no mask.  An input without nulls or a null scalar gives a
+ *   copy (with no type check, as in the reference); otherwise types differ -> DATA_TYPE.
+ * b2_replace_nulls_policy: PRECEDING: a null row takes the nearest valid value before it; FOLLOWING: after it.  A leading
+ *   (PRECEDING) or trailing (FOLLOWING) null run stays null.  An input with nulls gives an output with a mask whose null count
+ *   is that run's length; an input without nulls gives a copy.  A policy outside the enum -> LOGIC.
+ * b2_replace_nans / _scalar: FLOAT32 / FLOAT64 (any other type -> LOGIC, also empty).  A NaN row (valid) takes the
+ *   replacement's value and validity; a null row stays null.  The output has a mask when the input has nulls or the replacement
+ *   has a mask (the scalar form: always).  Sizes or types differ -> LOGIC.
+ * b2_find_and_replace_all: rows equal (C++ ==: -0.0 == +0.0, NaN equals nothing) to values_to_replace[j] take
+ *   replacement_values[j], the first such j among duplicates; a null replacement nulls the row; null rows stay null.  The output
+ *   has a mask exactly when the input or replacement_values has nulls.  Errors: sizes of the two value columns differ -> LOGIC;
+ *   any type differs -> DATA_TYPE; values_to_replace has nulls -> LOGIC.  An empty argument gives a copy.
+ * b2_clamp: x < lo -> lo_replace, x > hi -> hi_replace (C++ < and >: NaN is never clamped, -0.0 is not below +0.0); a null lo
+ *   or hi bound is not applied.  The output's mask is a copy of the input's.  Errors, in order: lo / hi, lo_replace /
+ *   hi_replace or lo / lo_replace types differ -> DATA_TYPE; both bounds null or an empty input -> a copy; a valid bound with a
+ *   null replacement -> LOGIC; input and lo types differ -> DATA_TYPE.  cudf::clamp(input, lo, hi) passes lo and hi as their
+ *   own replacements.
+ * b2_normalize_nans_and_zeros (/_inplace: over the view's own data): every NaN becomes quiet_NaN()'s bit pattern and -0.0
+ *   becomes +0.0; the mask and null count are the input's.  FLOAT32 / FLOAT64 only, else LOGIC (an empty input: a copy / no-op).
+ * Undefined values (as in the reference; no result depends on them): values under null bits.
+ * Decimal, dictionary, string and nested inputs -> DATA_TYPE (this library holds no such column). */
+enum { B2_REPLACE_PRECEDING = 0, B2_REPLACE_FOLLOWING = 1 };
+B2_API b2_status b2_replace_nulls(const b2_column_view* input, const b2_column_view* replacement, b2_stream stream, b2_column** out);
+B2_API b2_status b2_replace_nulls_scalar(const b2_column_view* input, const b2_scalar* replacement, b2_stream stream, b2_column** out);
+B2_API b2_status b2_replace_nulls_policy(const b2_column_view* input, int32_t policy, b2_stream stream, b2_column** out);
+B2_API b2_status b2_replace_nans(const b2_column_view* input, const b2_column_view* replacement, b2_stream stream, b2_column** out);
+B2_API b2_status b2_replace_nans_scalar(const b2_column_view* input, const b2_scalar* replacement, b2_stream stream, b2_column** out);
+B2_API b2_status b2_find_and_replace_all(const b2_column_view* input, const b2_column_view* values_to_replace,
+                                         const b2_column_view* replacement_values, b2_stream stream, b2_column** out);
+B2_API b2_status b2_clamp(const b2_column_view* input, const b2_scalar* lo, const b2_scalar* lo_replace, const b2_scalar* hi,
+                          const b2_scalar* hi_replace, b2_stream stream, b2_column** out);
+B2_API b2_status b2_normalize_nans_and_zeros(const b2_column_view* input, b2_stream stream, b2_column** out);
+B2_API b2_status b2_normalize_nans_and_zeros_inplace(const b2_column_view* in_out, b2_stream stream);
+
 /* Two-phase form of b2_partition for the fused partition + exchange: the plan holds the bucket id and the
  * stable in-bucket rank of every row; out_counts[b] = rows of bucket b.  b2_partition_scatter then writes one
  * fixed-width column straight to P destination base addresses — local buffers or PEER device memory mapped with

@@ -1132,7 +1132,8 @@ __global__ void __launch_bounds__(FIX_THREADS) segment_fix_kernel(pass_args a, i
 //   2. order each bucket directly: a row's place is its bucket's start + the number of the bucket's rows with a smaller
 //      (key, local row), so equal keys keep their input order: the stable sort, the hybrid plan's order row for row;
 //   3. write: the payload window (in L2 from a prefetch issued with the key load) replaces the dead keys in shared memory
-//      by a second bulk copy, and every output row is written coalesced from there.
+//      by a second bulk copy (estimated windows: issued before the walk of step 2, which then no longer reads the keys), and
+//      every output row is written coalesced from there.
 // A range longer than RANGE_CAP rows, or a bucket longer than RANGE_BUCKET_CAP rows (many equal or clustered keys), raises
 // ctl->overflow (the host reruns without the range tier).
 // Threads per CTA: 2^9 on the exact plan, 2^10 with estimated windows. Either way one CTA fills an SM's shared memory; the
@@ -1147,6 +1148,11 @@ constexpr int RANGE_BUCKETS     = 1 << RANGE_BUCKET_BITS;
 constexpr int RANGE_BUCKET_CAP  = FIX_HALO;  // rows of one bucket: each row compares its key with all of them
 constexpr int RANGE_SLOTS       = RANGE_BUCKETS + RANGE_BUCKETS / 32;  // padded counter layout of range_sort_kernel<VT, true>
 constexpr int RANGE_WALK_ROWS   = 4;  // rows of one thread whose bucket walks run side by side (estimated windows)
+// Unrolled walk steps of a group of RANGE_WALK_ROWS rows (estimated windows); a longer bucket finishes its row in a tail loop.
+// At 1e9 uniform keys a row's bucket holds 1 + Poisson(1.86) rows, 2.86 on average, and more than 4 for ~12 % of the rows;
+// a warp's 128 rows span ~45 buckets, whose largest (~6.4 rows) bounded the loop before. The phase probe (DESIGN §4.1) put
+// the walk at 6.62 us per range with 4 steps, 6.89 with 5 and 8.52 with the loop as long as the largest bucket.
+constexpr uint32_t RANGE_WALK_STEPS = 4;
 // Estimated windows: a bucket order entry is (16-bit key digest << 15 | local row), local rows < RANGE_CAP = 2^14.
 constexpr uint32_t RANGE_ROW_MASK = (1u << 15) - 1;
 
@@ -1425,34 +1431,48 @@ __global__ void __launch_bounds__(1 << range_log_threads<EST>, 1) range_sort_ker
   // ---- 2. the row at bucket position p goes to bucket start + #{bucket rows with a smaller (key, local row)} --------------
   // (the counters now hold the bucket ends; consecutive positions share buckets, so a warp's walks are mostly broadcasts)
   uint32_t pk[IPT];  // destination | local row << 16
+  range_window vw{0, false};
   if constexpr (EST) {
+    // The walk reads the keys only for each row's bucket bounds (and for the rare whole-key rank). With a payload, every thread
+    // first keeps the bounds of its rows (start | end << 16, in the slot pk takes later); the keys are then dead, and the payload
+    // window replaces them while the walk runs instead of behind it. The whole-key rank then reads the keys from the input.
+#pragma unroll
+    for (int i = 0; i < IPT; ++i) {
+      if (tid + RT * i >= m) break;
+      const uint32_t b = bucket(sk[s_ord[tid + RT * i] & RANGE_ROW_MASK]);
+      pk[i] = (b ? s_cnt[slot(b - 1)] : 0u) | s_cnt[slot(b)] << 16;
+    }
+    const UK* kw_rank = sk;
+    if (a.pairs) {
+      __syncthreads();
+      vw = range_window_load<RT>(s_vals, vin, s, m, mbar_v);
+      kw_rank = keys;
+    }
     // A row's place in its bucket is the number of the bucket's entries with a smaller digest, unless another row shares its
     // digest: that bucket is ranked again by whole keys (out of line: the unrolled walk must stay small enough for the
     // instruction cache). Entries and the bounds lo / hi lie in [0, 2^31], so the sign bit of eq - lo (eq - hi) says whether
     // eq's digest is smaller than (at most) this row's: one subtraction and one shift-add per count. The rows go in groups of
-    // RANGE_WALK_ROWS: the entry, key and counter loads of a group issue together, and one loop as long as the group's largest
-    // bucket walks its buckets side by side, each read clamped to its bucket's last entry, whose extra reads are subtracted
-    // behind the loop. Rows past m walk the one-entry bucket [0, 1) and are not written.
+    // RANGE_WALK_ROWS: RANGE_WALK_STEPS unrolled steps walk their buckets side by side, each read clamped to its bucket's last
+    // entry, whose extra reads are subtracted behind them. A bucket longer than that finishes its row alone (a warp waits for
+    // its longest such tail, per row of the group). Rows past m walk the one-entry bucket [0, 1) and are not written.
 #pragma unroll
     for (int i0 = 0; i0 < IPT; i0 += RANGE_WALK_ROWS) {
       if (tid + RT * i0 >= m) break;
       uint32_t e[RANGE_WALK_ROWS], start[RANGE_WALK_ROWS], end[RANGE_WALK_ROWS];
 #pragma unroll
       for (int g = 0; g < RANGE_WALK_ROWS; ++g) e[g] = tid + RT * (i0 + g) < m ? s_ord[tid + RT * (i0 + g)] : 0u;
-      uint32_t len = 0;
 #pragma unroll
       for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
         const bool in = tid + RT * (i0 + g) < m;
-        const uint32_t b = bucket(sk[e[g] & RANGE_ROW_MASK]);
-        end[g] = in ? s_cnt[slot(b)] : 1u;
-        start[g] = in && b ? s_cnt[slot(b - 1)] : 0u;
-        len = max(len, end[g] - start[g]);
+        start[g] = in ? pk[i0 + g] & 0xffffu : 0u;
+        end[g] = in ? pk[i0 + g] >> 16 : 1u;
       }
       // entries of a smaller digest lie below lo, of at most this row's digest below hi
       auto lo = [&](int g) { return e[g] & ~RANGE_ROW_MASK; };
       auto hi = [&](int g) { return (e[g] & ~RANGE_ROW_MASK) + RANGE_ROW_MASK + 1; };
       uint32_t lt[RANGE_WALK_ROWS] = {}, le[RANGE_WALK_ROWS] = {};
-      for (uint32_t q = 0; q < len; ++q) {
+#pragma unroll
+      for (uint32_t q = 0; q < RANGE_WALK_STEPS; ++q) {
 #pragma unroll
         for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
           const uint32_t eq = s_ord[min(start[g] + q, end[g] - 1)];
@@ -1462,12 +1482,21 @@ __global__ void __launch_bounds__(1 << range_log_threads<EST>, 1) range_sort_ker
       }
 #pragma unroll
       for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
-        const uint32_t extra = len - (end[g] - start[g]);
+#pragma unroll 1
+        for (uint32_t q = start[g] + RANGE_WALK_STEPS; q < end[g]; ++q) {
+          const uint32_t eq = s_ord[q];
+          lt[g] += (eq - lo(g)) >> 31;
+          le[g] += (eq - hi(g)) >> 31;
+        }
+      }
+#pragma unroll
+      for (int g = 0; g < RANGE_WALK_ROWS; ++g) {
+        const uint32_t extra = RANGE_WALK_STEPS - min(end[g] - start[g], RANGE_WALK_STEPS);
         const uint32_t eq = s_ord[end[g] - 1];
         lt[g] -= extra * ((eq - lo(g)) >> 31);
         le[g] -= extra * ((eq - hi(g)) >> 31);
         const uint32_t r = e[g] & RANGE_ROW_MASK;
-        if (le[g] - lt[g] > 1u) lt[g] = range_rank_keys(s_ord, sk, start[g], end[g], r, sk[r]);
+        if (le[g] - lt[g] > 1u) lt[g] = range_rank_keys(s_ord, kw_rank, start[g], end[g], r, kw_rank[r]);
         pk[i0 + g] = (start[g] + lt[g]) | r << 16;
       }
     }
@@ -1494,8 +1523,7 @@ __global__ void __launch_bounds__(1 << range_log_threads<EST>, 1) range_sort_ker
   RANGE_PROBE_STAMP(5);
 
   // ---- 3. sorted local rows -> s_perm; rows written in order from shared memory ----------------------------------------------
-  range_window vw{0, false};
-  if (a.pairs) vw = range_window_load<RT>(s_vals, vin, s, m, mbar_v);
+  if (!EST && a.pairs) vw = range_window_load<RT>(s_vals, vin, s, m, mbar_v);
 #pragma unroll
   for (int i = 0; i < IPT; ++i) {
     if (tid + RT * i >= m) break;

@@ -605,6 +605,55 @@ using tile_384x16      = tile_shape<384, 16, 2>;        // 8-byte keys: row ids,
 using tile_512x16      = tile_shape<512, 16, 1>;        // 1-, 2- and 4-byte keys
 using tile_512x20_bulk = tile_shape<512, 20, 1, true>;  // 8-byte keys carrying 8-byte payloads
 
+// BULK passes run one CTA per SM with nothing beside it, so a tile's 80 KB key copy would otherwise wait on HBM with the SM idle
+// (a third of the tile: DESIGN.md §4.1). Each tile's first look-back lane, idle until S2, bulk-prefetches into L2 the keys of
+// the tile KEY_PREFETCH_TILES ids ahead. Tiles are claimed in order at ~8 per µs over 132 SMs, so that tile starts ~3 µs
+// later, about the time its copy takes from HBM: its copy then reads L2. Measured on the H100 at 8 / 16 / 24 / 32 / 48 / 132
+// tiles ahead: 24 is the fastest, 16 and 32 are within 0.06 ms per pass of it; 132 tiles (10.5 MB in flight) is slower than
+// no prefetch, since the lines are evicted by the running tiles' scattered writes before they are read. Prefetching the
+// payload as well is slower too.
+constexpr uint32_t KEY_PREFETCH_TILES = 24;
+
+// Phase probe of onesweep_kernel (scripts/onesweep_probe.py), compiled only with -DB2_ONESWEEP_PROBE: ranking thread 0 (and
+// the first look-back lane for the look-back stamp) of the CTA that runs tile t writes clock64() at each phase boundary to
+// g_onesweep_probe[slot][phase][t], slot 0 for the pass that reads the raw keys and 1 for the others, and its SM id behind the
+// stamps. ONESWEEP_PROBE(...) expands to its argument only in that build: the shipped SASS is the same with and without it.
+#ifdef B2_ONESWEEP_PROBE
+constexpr int ONESWEEP_PROBE_TILES  = 1 << 17;
+// entry, tile id known, keys landed, S1, S1b, S2, ranked and staged, S4, look-back done, keys written, payload landed,
+// payload written
+constexpr int ONESWEEP_PROBE_STAMPS = 12;
+__device__ long long g_onesweep_probe[2][ONESWEEP_PROBE_STAMPS + 1][ONESWEEP_PROBE_TILES];
+void* g_onesweep_probe_ptr()
+{
+  void* p = nullptr;
+  cudaGetSymbolAddress(&p, g_onesweep_probe);
+  return p;
+}
+__device__ __forceinline__ long long onesweep_probe_clock()
+{
+  long long v;
+  asm volatile("mov.u64 %0, %%clock64;" : "=l"(v)::"memory");  // not moved across the phase's memory operations
+  return v;
+}
+__device__ __forceinline__ void onesweep_probe_put(int slot, int i, uint32_t tile, long long v)
+{
+  if (tile < (uint32_t)ONESWEEP_PROBE_TILES) g_onesweep_probe[slot][i][tile] = v;
+}
+__device__ __forceinline__ long long onesweep_probe_smid()
+{
+  uint32_t s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
+#define ONESWEEP_PROBE(...) __VA_ARGS__
+#else
+#define ONESWEEP_PROBE(...)
+#endif
+// one stamp by the thread `who` of the current tile
+#define ONESWEEP_STAMP_BY(who, i) ONESWEEP_PROBE(if (tid == (who)) onesweep_probe_put(pl.key_src != 0, i, tile, onesweep_probe_clock());)
+#define ONESWEEP_STAMP(i) ONESWEEP_STAMP_BY(0, i)
+
 // EST (64-bit raw keys, range sort with estimated bases): digit d owns rows [d * est_cap, (d + 1) * est_cap) of the output (overflow
 // check as MIX), the last tile publishes every digit's end, and the first pass ORs (key ^ first key) into ctl->vary; with est_tiles
 // the tiles come from that table (the windows of the first pass) instead of one contiguous portion.
@@ -621,6 +670,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 
   const pass_plan pl = a.ctl->plan[a.pass];
   if (pl.trivial) return;
+  ONESWEEP_PROBE(const long long probe_entry = onesweep_probe_clock();)
 
   B2_DYNAMIC_SMEM(smem_raw);
   constexpr int STAGE_W = sizeof(UK) > sizeof(VT) ? sizeof(UK) : sizeof(VT);  // staging holds keys, then the payload
@@ -685,6 +735,11 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       nlim      = tile_base + tile_n;
     }
   }
+  ONESWEEP_PROBE(if (tid == 0) {
+    onesweep_probe_put(pl.key_src != 0, 0, tile, probe_entry);
+    onesweep_probe_put(pl.key_src != 0, ONESWEEP_PROBE_STAMPS, tile, onesweep_probe_smid());
+  })
+  ONESWEEP_STAMP(1);
   const bool full = tile_n == (uint32_t)TILE;
   const uint32_t pad = (uint32_t)TILE - tile_n;      // padding items sit at the end of digit 255
   const int shift = a.pass * RADIX_BITS;
@@ -692,6 +747,25 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 
   if (!ranker) {
     // ================================ look-back warp ==============================================
+    if constexpr (BULK && !EMU_BUILD) {
+      if (tid == THREADS) {  // keys of a later tile into L2 (KEY_PREFETCH_TILES): only full, 16-byte aligned tiles take bulk copies
+        const uint32_t tp = tile + KEY_PREFETCH_TILES, ntiles = (a.portion_n + TILE - 1) / TILE;
+        uint32_t base = tp * (uint32_t)TILE, rows = 0;
+        if (EST && a.est_tiles != nullptr) {
+          if (tp < ntiles + RADIX) {  // the tile table's size (run_est_range)
+            const uint2 e = a.est_tiles[tp];
+            base = e.x;
+            rows = e.y & 0x7fffffffu;
+          }
+        } else if (tp < ntiles) {
+          rows = min((uint32_t)TILE, a.portion_n - base);
+        }
+        const UK* ks = static_cast<const UK*>(pl.key_src == 0 ? a.key_bufs[0] : (pl.key_src == 1 ? a.key_bufs[1] : a.key_bufs[2])) +
+                       a.portion_start + base;
+        if (rows == (uint32_t)TILE && (reinterpret_cast<uintptr_t>(ks) & 15) == 0)
+          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(ks), "r"((uint32_t)(sizeof(UK) * TILE)) : "memory");
+      }
+    }
     cta_barrier(THREADS + 32 * LBW);  // (S2) agg[tile][*] written by the rankers; s_cnt = {count, tile-local start}
     const int d0 = ((warp - NWARPS) * 32 + lane) * DPL;
     uint32_t cnt[DPL], loc[DPL], excl[DPL];
@@ -760,6 +834,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       s_off[d0 + j] = g + excl[j] - loc[j];
       if (last_of_portion) a.ctl->base[a.portion_parity ^ 1][a.pass][d0 + j] = g + excl[j] + cnt[j];
     }
+    ONESWEEP_STAMP_BY(THREADS, 8);
     cta_barrier(THREADS + 32 * LBW);  // (S4) offsets ready
     return;
   }
@@ -826,6 +901,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       }
     }
   }
+  ONESWEEP_STAMP(2);
 
   // digit of a key: a byte of it, or (RANGE) the number of splitters <= key — padding items (all-ones key) land in the last bucket
   auto digit_of = [&](UK k) -> unsigned {
@@ -855,6 +931,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
   uint32_t* my_hist = s_whist + warp * RADIX;
   const int distinct = warp_digit_counts<IPT>(digit_at, IPT, lane, my_hist);
   ranker_barrier(THREADS);  // (S1)
+  ONESWEEP_STAMP(3);
   if constexpr (EST) {
     if (tid == 0 && pl.key_src == 0) {  // one global atomic per CTA
       const unsigned long long v = ((unsigned long long)s_misc[11] << 32) | s_misc[10];
@@ -879,6 +956,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     tstart = inc - padded;
   }
   ranker_barrier(THREADS);  // (S1b)
+  ONESWEEP_STAMP(4);
   if (tid < RADIX) {
     uint32_t woff = 0;
 #pragma unroll
@@ -891,6 +969,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     for (int w = 0; w < NWARPS; ++w) s_whist[w * RADIX + tid] += tstart;
   }
   cta_barrier(THREADS + 32 * LBW);  // (S2) releases the look-back warps; warp offsets final
+  ONESWEEP_STAMP(5);
 
   // ---- rank within warp (stable): peer masks + running per-warp digit offsets ---------------------
   uint32_t pos[IPT];
@@ -902,6 +981,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
 #pragma unroll
     for (int i = 0; i < IPT; ++i) s_dig[pos[i]] = (uint8_t)dg[i];
   }
+  ONESWEEP_STAMP(6);
   // row ids are fetched only now (their registers replace the dead key registers); the loads
   // overlap with the key write-out below
   VT idx[IPT];
@@ -934,6 +1014,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
     }
   }
   cta_barrier(THREADS + 32 * LBW);  // (S4) keys staged, scatter offsets ready
+  ONESWEEP_STAMP(7);
 
   const bool write_keys = !(a.pairs && pl.last) || a.keep_keys || pl.hybrid;
   UK* kdst = static_cast<UK*>(const_cast<void*>(pl.key_dst == 1 ? a.key_bufs[1] : a.key_bufs[2]));
@@ -961,10 +1042,12 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
       kdst[dst[j]] = k;
     }
   }
+  ONESWEEP_STAMP(9);
   if (a.pairs) {
     ranker_barrier(THREADS);
 #pragma unroll
     for (int i = 0; i < IPT; ++i) s_vals[pos[i]] = idx[i];
+    ONESWEEP_STAMP(10);
     ranker_barrier(THREADS);
     VT* idst = reinterpret_cast<VT*>(pl.idx_dst == 0 ? a.idx_bufs[0] : (pl.idx_dst == 1 ? a.idx_bufs[1] : a.idx_bufs[2]));
 #pragma unroll
@@ -976,6 +1059,7 @@ __global__ void __launch_bounds__(Shape::threads + 32 * LBW, Shape::min_blocks) 
         if (q < tile_n && (!(MIX || EST) || dst[j] != 0xFFFFFFFFu)) idst[dst[j]] = s_vals[q];
       }
     }
+    ONESWEEP_STAMP(11);
   }
 }
 
@@ -2685,6 +2769,21 @@ column_ptr sort_single_column(const b2_column_view& col, bool ascending, cudaStr
 }
 
 }  // namespace b2
+
+#ifdef B2_ONESWEEP_PROBE
+// scripts/onesweep_probe.py: clears / copies out the phase stamps of the last onesweep_kernel launches (row-major
+// [2][ONESWEEP_PROBE_STAMPS + 1][ONESWEEP_PROBE_TILES] int64).
+extern "C" B2_API int b2_onesweep_probe_reset(void)
+{
+  return (int)cudaMemset(b2::g_onesweep_probe_ptr(), 0, sizeof(b2::g_onesweep_probe));
+}
+extern "C" B2_API int b2_onesweep_probe_read(long long* out, int* stamps, int* tiles)
+{
+  *stamps = b2::ONESWEEP_PROBE_STAMPS;
+  *tiles  = b2::ONESWEEP_PROBE_TILES;
+  return (int)cudaMemcpy(out, b2::g_onesweep_probe_ptr(), sizeof(b2::g_onesweep_probe), cudaMemcpyDeviceToHost);
+}
+#endif
 
 #ifdef B2_RANGE_PROBE
 // scripts/range_probe.py: clears / copies out the phase stamps of the last range_sort_kernel launches (row-major
